@@ -10,11 +10,13 @@ GPU, bf16).
     python bench.py --global-batch 16 ...       # strong scaling: the global batch is fixed and sharded over the ranks
     python bench.py --sweep                     # every BASELINE config + the keypoint batch sweep, one JSON line each
     python bench.py --impl reference ...        # the reference's own PLMSSampler + UNetModel on the host cores
+    python bench.py --dump-outputs DIR ...      # also write the last timed step's final latents as DIR/latent.npy
 
 One "step" = one full `PLMSSampler.sample(S=50)` of one batch = 102 UNet forwards per image (cond + uncond
 x (50 + 1)); weights are seeded random of the SD-1.4 + GLIGEN architecture (no checkpoints offline), inputs
 are synthetic CLIP/grounding embeddings (SURVEY 8d).  `value` times the loop with inputs already resident in
-HBM; `e2e` times the same public call with inputs in pinned HOST memory and the final latent read back.
+HBM; `e2e` times the same public call with inputs in pinned HOST memory and the final latent read back.  Every sampled
+batch starts from the same seeded noise, so runs with the same arguments compute the same latents.
 """
 from __future__ import annotations
 
@@ -64,7 +66,11 @@ def parse(argv=None):
     ap.add_argument("--no-kernel-pass", action="store_true")
     ap.add_argument("--sweep", action="store_true", help="all BASELINE configs + keypoint batch sweep (1 GPU); one JSON line each")
     ap.add_argument("--ref-budget-s", type=float, default=200.0, help="reference arm: wall-clock budget that sizes its bounded sample")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the final latents of the last timed step (fp32, what PLMSSampler.sample returns) as DIR/latent.npy")
     args = ap.parse_args(argv)
+    if args.dump_outputs:
+        args.dump_outputs = os.path.abspath(args.dump_outputs)      # run_ours may chdir before it writes
     if args.preset:
         pr = PRESETS[args.preset]
         given = argv if argv is not None else sys.argv
@@ -159,7 +165,7 @@ class ClockSampler:
 def _thread_candidates():
     """Thread counts worth trying for the CPU arm, ascending: 16, 32, the physical cores, all logical CPUs (torch's
     intra-op parallelism over 100+ hyper-threads is far slower than over a few dozen cores for these layer sizes:
-    measured on the B200 host 49 s per forward at 128 threads against 5.4 s at 32)."""
+    measured once at 49 s per forward at 128 threads against 5.4 s at 32 on a 128-thread host)."""
     n = os.cpu_count() or 1
     cand = {n, min(32, n), min(16, n)}
     try:
@@ -379,6 +385,7 @@ def run_ours(args, world, rank, local_rank, dev, quiet_extras=False):
     def one_image_batch(from_host: bool):
         if B == 0:
             return None
+        torch.manual_seed(1234 + rank)                 # the initial noise x_T of every step is the same seeded draw
         if from_host:
             t = {k: v.to(dev, non_blocking=True) for k, v in pinned.items()}
             bt = {k: v.to(dev, non_blocking=True) for k, v in pinned_batch.items()}
@@ -395,12 +402,14 @@ def run_ours(args, world, rank, local_rank, dev, quiet_extras=False):
             torch.distributed.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(n, from_host):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(n):
-            one_image_batch(from_host)
+            last["latent"] = one_image_batch(from_host)
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
@@ -420,6 +429,10 @@ def run_ours(args, world, rank, local_rank, dev, quiet_extras=False):
     clocks.start()
     l0 = eng.kernel_launches
     ms = timed(args.steps, False)
+    if args.dump_outputs and last.get("latent") is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        name = "latent.npy" if world == 1 else f"latent_rank{rank}.npy"
+        np.save(os.path.join(args.dump_outputs, name), last["latent"].float().cpu().numpy())
     launches = eng.kernel_launches - l0 + (args.steps * (S + 1) if B else 0)          # + the fused sampler-update kernels
     clk = clocks.stop()
     one_image_batch(True)
@@ -438,8 +451,8 @@ def run_ours(args, world, rank, local_rank, dev, quiet_extras=False):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1.4 PFLOP/s sustained (of fallback)"
+        peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "H100 SXM data sheet, dense bf16 989 TFLOP/s"
         roof = {"bound": "tensor", "unit": "TFLOP/s", "peak": peak_tf, "peak_source": peak_src, "traffic": None}
         kernel_shares = None
         if not args.no_kernel_pass and B > 0:
@@ -455,23 +468,10 @@ def run_ours(args, world, rank, local_rank, dev, quiet_extras=False):
                                  "gbs": round(a[1] / (a[2] * 1e-3) / 1e9, 1) if a[1] and a[2] else None} for k, a in agg.items()}
             # dominant kernel = gemm_tc_kernel (linear + 1x1 + implicit 3x3 conv): algorithmic flops per launch
             # / average CUDA-event launch duration, both from this live pass
-            roof.update({"kernel": "gemm_tc_kernel (tcgen05 GEMM + implicit-GEMM conv3x3)",
+            roof.update({"kernel": "gemm_tc_kernel (wgmma GEMM + implicit-GEMM conv3x3)",
                          "achieved": tc_fl / (tc_ms * 1e-3) / 1e12, "frac": tc_fl / (tc_ms * 1e-3) / 1e12 / peak_tf,
                          "flops_per_launch": tc_fl / max(tc_n, 1), "avg_launch_ms": tc_ms / max(tc_n, 1), "launches_per_forward": tc_n,
                          "forward_ms_sum_of_ops": tot_ms, "op_timing": "each op replayed from its own CUDA graph (GPU time, no host issue time)"})
-            if not quiet_extras:
-                os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-                with open(os.path.join(ROOT, "gpurun_out", "bench_per_op.json"), "w") as f:
-                    json.dump([dict(name=n, kind=k, gflop=fl / 1e9, mbytes=by / 1e6, ms=m) for n, k, fl, by, m in per_op], f)
-        for tname in ("r2_gemm_dram_traffic.json", "r1_gemm_dram_traffic.json"):
-            tpath = os.path.join(ROOT, "profiles", tname)
-            if os.path.exists(tpath):                  # measured with ncu (bench.py cannot run under a profiler itself)
-                tr = json.load(open(tpath))
-                roof["traffic"] = tr["dram_bytes_read_per_launch"] + tr["dram_bytes_write_per_launch"]
-                roof["traffic_note"] = ("dram__bytes_read.sum + dram__bytes_write.sum per gemm_tc_kernel launch, mean of "
-                                        f"{tr['launches']} launches (profiles/{tname}); algorithmic minimum "
-                                        f"{tr['algorithmic_bytes_per_launch']:.3g} B/launch - L2 (126 MB) keeps producer->consumer activations off DRAM")
-                break
         roof["whole_step_achieved"] = f_img * value / world / 1e12
         roof["whole_step_frac"] = roof["whole_step_achieved"] / peak_tf
         cpu = None
@@ -483,7 +483,7 @@ def run_ours(args, world, rank, local_rank, dev, quiet_extras=False):
                 "config": {"workload": workload_string(args.config, cfg, args, B if not strong else f"{args.global_batch} global / {world}", atype),
                            "forwards_per_image": 2 * (S + 1), "cfg_batching": "cond+uncond as one 2B pass",
                            "parallelism": f"dp{world} (sample sharding, no per-step collective)",
-                           "l2": "working set (2.1 GB bf16 weights + activations) >> 126 MB L2; no explicit flush",
+                           "l2": "working set (2.1 GB bf16 weights + activations) >> 50 MB L2; no explicit flush",
                            "weights_broadcast": {"bytes": sent, "seconds": round(t_bc, 3), "what": "packed bf16 arena + fp32 vectors"} if world > 1 else None,
                            "algorithmic_tflop_per_image": f_img / 1e12},
                 "e2e": {"value": e2e, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "ms_per_step": ms_e2e / args.steps},

@@ -1,4 +1,4 @@
-"""gligen_b200: Blackwell-native (sm_100a) GLIGEN denoising engine.
+"""gligen_b200: Hopper-native (sm_90a) GLIGEN denoising engine.
 
 Host code is Python/PyTorch (plumbing); every hot op is a hand-written CUDA kernel reached
 through the C-ABI library `libgligen_b200.so` (see include/gligen_b200.h).

@@ -1,8 +1,8 @@
-"""Build libgligen_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libgligen_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m gligen_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the objects under _build/ are git-ignored build products.
 """
 from __future__ import annotations
 
@@ -16,10 +16,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libgligen_b200.so")
-SOURCES = ["capi.cu", "engine_capi.cu", "tma_host.cu", "gemm_tc.cu", "attention.cu", "attention_tc.cu", "attention_short_tc.cu", "attention_tc2.cu", "attention_tc3.cu", "norm.cu", "elementwise.cu", "frontend.cu"]
+SOURCES = ["capi.cu", "engine_capi.cu", "tma_host.cu", "gemm_tc.cu", "attention.cu", "norm.cu", "elementwise.cu", "frontend.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -48,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB
     if not os.path.exists(NVCC):
         if os.path.exists(LIB):
-            return LIB           # GPU box without a matching stamp: use the prebuilt library
+            return LIB           # no compiler on this machine: use the library built where one was
         raise RuntimeError(f"nvcc not found at {NVCC} and no prebuilt {LIB}")
 
     def compile_one(src):
@@ -66,7 +66,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [NVCC, "-shared", "-o", LIB + ".tmp", *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [NVCC, "-shared", "-o", LIB + ".tmp", *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}{r.stderr}")

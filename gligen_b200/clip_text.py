@@ -8,7 +8,7 @@ reference tree): CLIPTextTransformer = token + position embeddings, 12 pre-Layer
 position of the highest token id (the EOT token).  Restated in oracle/clip_oracle.py and pinned against the installed
 transformers' CLIPTextModel.
 
-Here: one gather kernel for the embeddings, LayerNorm rows, fused-QKV glg_gemm, the short-key tcgen05 attention kernel with
+Here: one gather kernel for the embeddings, LayerNorm rows, fused-QKV glg_gemm, the short-key attention kernel with
 its causal mask, out-projection / fc2 GEMMs with the residual add in the epilogue, fc1 with the quick_gelu epilogue.
 bf16 activations and weights, fp32 accumulation / statistics, fp32 output.
 """

@@ -25,7 +25,7 @@ int pdl_mode() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("GLG_PDL");
-    v = e ? atoi(e) : 0;            // measured on B200: no gain for this launch mix (profiles/), so opt-in
+    v = e ? atoi(e) : 0;            // opt-in
   }
   return v;
 }

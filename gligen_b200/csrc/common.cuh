@@ -1,5 +1,5 @@
-// Shared device-side helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM, small math.
-// Everything here is inline PTX written for sm_100a (no CUTLASS dependency).
+// Shared device-side helpers for the sm_90a kernels: mbarrier, TMA, wgmma, clusters, small math.
+// Everything here is inline PTX written for sm_90a (no CUTLASS dependency).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -16,7 +16,7 @@ __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)
 // With GLG_PDL=1 every kernel is launched with cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel
-// in the stream may be scheduled (and run its prologue: barrier init, TMEM alloc, descriptor prefetch) while this
+// in the stream may be scheduled (and run its prologue: barrier init, descriptor prefetch) while this
 // one drains; pdl_wait() blocks until the previous grid has completed and its memory is visible, so it must precede
 // the first access to global data.  Without the launch attribute both are no-ops.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -67,7 +67,9 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 // Wait with a watchdog: a protocol bug traps (-> cudaErrorLaunchFailure at the next sync) instead of
-// hanging the GPU box.  The watchdog only runs on the slow path.
+// hanging the GPU.  The watchdog only runs on the slow path.  VERBOSE = false leaves out the printf: a function call
+// between wgmma.mma_async and its wait makes ptxas serialise the warpgroup MMAs.
+template <bool VERBOSE = true>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 #pragma unroll 1
   for (int i = 0; i < 256; ++i)           // common case: the phase completes within a few (HW-suspended) polls - no timer read on this path
@@ -78,7 +80,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     for (int i = 0; i < 64; ++i)          // the timer read is slow: keep it off the wake-up path
       if (mbar_try_wait(bar, parity)) return;
     if (globaltimer_ns() - t0 > 4000000000ull) {  // 4 s
-      printf("glg: mbarrier timeout block %d thread %d bar %u parity %u\n", blockIdx.x, threadIdx.x, bar, parity);
+      if (VERBOSE) printf("glg: mbarrier timeout block %d thread %d bar %u parity %u\n", blockIdx.x, threadIdx.x, bar, parity);
       __trap();
     }
   }
@@ -93,10 +95,8 @@ __device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
   mbar_wait(bar, parity);
 }
 
-// One leader lane of a fully converged warp.  The single-thread roles (TMA producer, MMA issuer) run the whole warp
-// through their loops and predicate the issue on this flag: a role entered as `if (lane == 0)` makes the compiler wrap
-// every UTCHMMA / UTCBAR / UTMALDG in an ELECT + BRA.U.ANY loop over "the active lanes" (~6 slow uniform-datapath
-// instructions each); with elect.sync the same instructions are emitted back to back, predicated.
+// One leader lane of a fully converged warp.  The single-thread TMA producer runs the whole warp through its loop and
+// predicates the issue on this flag, so the compiler does not wrap every UTMALDG in a loop over "the active lanes".
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -120,125 +120,66 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
+// ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R> __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same, with the A operand read from TMEM (128 lanes x K bf16 packed two per 32-bit column).
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128B swizzle, rows of 64 bf16 (=128 B),
-// 8-row core-matrix groups 1024 B apart (SBO).  (cute::UMMA::SmemDescriptor, version 1 = Blackwell.)
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, K-major operand, 128B swizzle, rows of 64 bf16 (=128 B), 8-row core-matrix groups
+// 1024 B apart (SBO); the tile base must be 1024-byte aligned.  Advancing K by 16 elements adds 32 B (= 2 in the
+// start-address field) inside the swizzle atom.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address  [0,14)
   d |= (uint64_t)1 << 16;                              // LBO (unused for swizzled K-major) [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;                    // SBO = 1024 B  [32,46)
-  d |= (uint64_t)1 << 46;                              // descriptor version = 1
-  d |= (uint64_t)2 << 61;                              // layout type = SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                              // layout type = SWIZZLE_128B [62,64)
   return d;
-}
-// MN-major operand (e.g. V[key][d] used as B[K=key][N=d]): rows of 64 bf16 along MN (128 B), one row per K
-// index, 8-row groups 1024 B apart (SBO); further 64-wide MN atoms follow at LBO bytes.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;    // LBO: byte offset between 64-element MN atoms
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Instruction descriptor for kind::f16: BF16 x BF16 -> F32, both operands K-major, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, bool b_mn_major = false) {
-  return (b_mn_major ? (1u << 16) : 0u)   // B major: 0 = K, 1 = MN
-       | (1u << 4)                      // C format = F32
-       | (1u << 7)                      // A format = BF16
-       | (1u << 10)                     // B format = BF16
-       | ((uint32_t)(N >> 3) << 17)     // N / 8
-       | ((uint32_t)(M >> 4) << 24);    // M / 16
 }
 
-__device__ __forceinline__ uint32_t tmem_ld1(uint32_t taddr) {     // one 32-bit column of this thread's lane
+// ------------------------------------------------------------------ clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-// TMEM -> registers: 32 lanes x 32 columns of 32-bit; thread i of the warp receives lane (base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t mapa_cluster(uint32_t local_addr, uint32_t cta) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta));
+  return r;
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+// TMA load delivered to the same smem offset of every CTA in `mask`; each destination CTA's mbarrier at `bar`'s
+// offset receives the bytes it got
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, uint16_t mask) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ math
+// exp2 on the FMA / ALU pipes (Cody-Waite split + Taylor cubic on [-0.5, 0.5]: relative error 1.2e-4 mean, 7.9e-4 max at
+// |f| = 0.5, against 2e-3 for the bf16 rounding of P; tests/test_exp2_poly_cpu.py): the attention softmax can move a share
+// of its exponentials off the MUFU pipe (16 exp2 / clk / SM), which bounds it at small head dims.
+__device__ __forceinline__ float ex2_poly3(float x) {
+  x = fmaxf(x, -125.0f);
+  const float t = x + 12582912.0f;                 // 1.5 * 2^23: round(x) lands in the low mantissa bits
+  const float f = x - (t - 12582912.0f);
+  float p = fmaf(0.05550411f, f, 0.24022651f);
+  p = fmaf(p, f, 0.69314718f);
+  p = fmaf(p, f, 1.0f);
+  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
+}
 // x * sigmoid(x); __fdividef: 2 ulp, no IEEE-division slow path (a CALL per element in the epilogues)
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // CLIP's activation (transformers "quick_gelu": x * sigmoid(1.702 x))

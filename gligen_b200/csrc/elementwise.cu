@@ -350,7 +350,7 @@ __global__ void sampler_update_kernel(const float* __restrict__ x, const float* 
 namespace glg {
 // Row softmax of an fp32 score matrix -> bf16 probabilities (sum of a row = 1 before rounding): one CTA per row.
 // Used by the VAE decoder's single-head attention over H*W tokens (model.py:178-202), whose head dim (512) is too wide
-// for the flash kernels' TMEM budget: QK^T and P.V run as glg_gemm, the scores make one round trip through L2.
+// for the flash kernels' register-resident output tile: QK^T and P.V run as glg_gemm, the scores make one round trip through L2.
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ s, long long lds, bf16* __restrict__ p, long long ldp,
                                                           int cols, float scale_log2) {
   pdl_trigger();

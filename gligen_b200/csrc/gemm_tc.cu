@@ -1,30 +1,24 @@
-// tcgen05 / TMEM / TMA GEMM and implicit-GEMM 3x3 convolution for sm_100a.
+// wgmma / TMA GEMM and implicit-GEMM 3x3 convolution for sm_90a.
 //
-//   out[M,N] = epilogue( A[M,K] . W[N,K]^T )           bf16 operands, fp32 accumulation in TMEM
+//   out[M,N] = epilogue( A[M,K] . W[N,K]^T )           bf16 operands, fp32 accumulation in registers
 //
-// Persistent, warp-specialised, 20 warps per CTA:
-//   warp 0        : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warp 1        : MMA issuer    (tcgen05.mma, K=16 per instruction, up to 4 accumulator stages in TMEM)
-//   warps 2..3    : idle (keep the epilogue warps' index aligned with the TMEM lane quarters)
-//   warps 4..19   : epilogue      (tcgen05.ld 32x32b -> registers -> LayerNorm fold / bias / time-embedding row
-//                                  bias / SiLU / tanh-gate / residual / GEGLU -> bf16 -> 64B-swizzled smem -> TMA store);
-//                                  four warps per TMEM lane quarter, each taking every fourth 32-column chunk of the
-//                                  tile; residual chunks arrive by TMA, LayerNorm statistics are prefetched BEFORE the
-//                                  accumulator is ready.
+// Persistent, warp-specialised, three warpgroups per CTA (384 threads):
+//   warpgroup 0   : TMA producer (one elected lane of warp 0: cp.async.bulk.tensor -> 128B-swizzled smem ring,
+//                   mbarrier complete_tx); gives most of its registers to the consumers (setmaxnreg)
+//   warpgroups 1-2: consumers, each owning 64 rows of the 128 x BN tile: wgmma.mma_async m64nBNk16 on the smem
+//                   descriptors, fp32 accumulators in registers, then the epilogue straight from registers
+//                   (LayerNorm fold / bias / time-embedding row bias / SiLU / GELU / tanh-gate / residual / GEGLU ->
+//                   bf16 or fp32 global stores, per-row LayerNorm partial sums of what is stored)
 //
 // Two instantiations of the same code:
-//   CTA2 = false : one CTA per tile, tcgen05.mma.cta_group::1, tile 128 x BN.
-//   CTA2 = true  : a cluster of two CTAs (one TPC) per 256 x BN tile, tcgen05.mma.cta_group::2 issued by the
-//                  leader CTA; each CTA stages its own 128 rows of A and HALF of the B tile, the tensor core
-//                  reads both halves, so every operand byte fetched from L2 feeds twice the math.  These GEMMs
-//                  are L2->SM bandwidth bound (a 128 x 256 tile needs ~96 B/clk/SM against ~42 available,
-//                  B300_MICROARCH "LTS throughput"); the paired tile halves that.
+//   CTA2 = false : one CTA per 128 x BN tile.
+//   CTA2 = true  : a cluster of two CTAs per 256 x BN tile: each CTA stages its own 128 rows of A and loads HALF of the
+//                  B tile with a TMA multicast into both CTAs, so every weight byte fetched from L2 feeds two CTAs.
+//                  A stage is refilled only when the consumers of BOTH CTAs have released it (remote mbarrier arrives).
 //
 // B-resident mode (b_res): when a CTA's whole weight tile W[n_blk*BN .. +BN, 0..K) fits in shared memory next to a few
-// A stages (K*BN*2 bytes <= ~160 KB: the K = 320 / 640 projections), every CTA keeps ONE n-tile for its lifetime, loads
-// that weight tile once and streams only A tiles: L2 -> SM operand traffic per output tile drops from (128 + BN) to 128
-// rows per K step.  These short-K GEMMs are operand-delivery bound (ncu: tensor pipe 28 %, L2 -> SM at its ~60 B/clk/SM
-// limit), so this is worth up to (128 + BN) / 128 in time.
+// A stages (the K = 320 / 640 projections), every CTA keeps ONE n-tile for its lifetime, loads that weight tile once and
+// streams only A tiles.
 //
 // conv_mode: the A operand is gathered by a 4-D tiled tensor map over the NHWC activation
 // (C, W, H, B); for tap (dy,dx) the box origin is shifted by (dx-1, dy-1) and TMA's out-of-bounds
@@ -40,6 +34,7 @@
 
 #include "common.cuh"
 #include "internal.h"
+#include "wgmma.cuh"
 #include "../../include/gligen_b200.h"
 
 namespace glg {
@@ -57,378 +52,136 @@ struct GemmKParams {
   float* stats_out; int stats_slots;
   // batch-strided output rows: address = (row / orpb) * obs + (row % orpb) * ldc   (orpb == 0: uniform rows)
   int orpb; long long obs;
-  int wide;                       // 1: rows of out / residual are 32-byte aligned -> 256-bit global accesses
   // split-K: `splits` CTAs share one output tile, each reducing a contiguous range of K steps into its own fp32
   // slab ws[split][M][N]; splitk_reduce_kernel sums the slabs in a fixed order and applies the epilogue.
   int splits; float* ws;
   int stages;                     // depth of the smem ring (runtime: B-resident mode trades stages for the weight tile)
   int b_res;                      // 1: weights resident in smem, one n-tile per CTA for its lifetime
-  // epilogue data path through shared memory + TMA (see "epilogue data path" below)
-  int tma_out;                    // 0: per-thread global stores; 2 / 3: TMA stores with a 2-D / 3-D (batch-strided rows) tensor map
-  int tma_res;                    // 1: residual chunks arrive by TMA load into per-warp staging
-  unsigned epi_off;               // byte offset (from the tile base) of the epilogue staging area
   long long stats_stride;         // stats_out / ln_stats are SLOT-major: element (slot, row) at [slot * stride + row]
   long long ln_stride;
-  int dbg;                        // scripts/micro knock-outs (results are garbage, time is real): 1 no TMA loads, 2 no MMAs,
-                                  // 4 no epilogue work (barrier protocol only), 8 no output stores
 };
 
 template <int BN, bool CTA2> struct GemmCfg {
   static constexpr int BM = 128, BK = 64;
+  static constexpr int THREADS = 384;
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int BROWS = CTA2 ? BN / 2 : BN;                  // rows of W staged by one CTA
-  static constexpr int B_BYTES = BROWS * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int B_HALF = B_BYTES / 2;                         // CTA2: the share of B one CTA loads
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int MAX_STAGES = 12;
-  static constexpr int STAGES = (196 * 1024) / STAGE_BYTES > 8 ? 8 : (196 * 1024) / STAGE_BYTES;     // streaming mode
-  // accumulator stages in TMEM: short-K tiles are bound by the MMA <-> epilogue hand-off latency, so use as many
-  // stages as the 512 columns allow (BN=256: 2, 160: 3, <=128: 4)
-  static constexpr int ACC = (512 / BN) > 4 ? 4 : (512 / BN);
-  static constexpr int TMEM_COLS = (ACC * BN <= 128) ? 128 : (ACC * BN <= 256) ? 256 : 512;
   static constexpr int BAR_BYTES = 1024;                             // barriers live in FRONT of the tiles (runtime stage count)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + BAR_BYTES;
-  static constexpr int SMEM_MAX = 227 * 1024;                        // B-resident mode takes the whole SM
-  static constexpr int TILE_BYTES_MAX = SMEM_MAX - 1024 - BAR_BYTES;
-  static_assert(8 * (2 * MAX_STAGES + 2 * ACC + 1) + 8 <= BAR_BYTES, "barrier area");
-  static_assert(B_BYTES % 1024 == 0, "B stage must keep 1024-byte alignment of the next A stage");
+  static constexpr int SMEM_MAX = 227 * 1024;
+  static_assert(8 * (2 * MAX_STAGES + 1) <= BAR_BYTES, "barrier area");
+  static_assert(B_HALF % 1024 == 0, "each half of the B stage must keep the 1024-byte swizzle alignment");
 };
 
-// ---- cluster / cta_group::2 PTX ------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_cluster(uint32_t local_addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA loads whose completion bytes are credited to the LEADER CTA's mbarrier (peer bit of the address cleared)
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit -> arrive on the barrier at the same smem offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
+__device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+__device__ __forceinline__ void add2(float& a, float& b, const float* p) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); a += t.x; b += t.y; }
+
+__device__ __forceinline__ float act_f(int act, float v) {
+  if (act == GLG_ACT_SILU) return silu_f(v);
+  if (act == GLG_ACT_GELU) return gelu_erf_f(v);
+  if (act == GLG_ACT_QUICK_GELU) return quick_gelu_f(v);
+  return v;
 }
 
-// ---- epilogue data path --------------------------------------------------------------------------------------
-// In the epilogue a thread owns one accumulator ROW (TMEM lane).  Writing that row's 64-byte chunks straight to global
-// memory makes every warp-level store touch 32 different 128-byte lines: the LSU replays it ~32 x 2 cycles, and the
-// same for the residual reads and the LayerNorm partials.  For the short-K projections (K = 320: 1600 MMA cycles per
-// tile) those replays - ~6500 cycles per 128 x 160 tile - were the whole kernel time (measured: the same 22 us with or
-// without the weight tile resident in smem).  So every per-row global access of the epilogue goes through shared
-// memory and the TMA instead: a warp stages its [32 rows x 32 columns] bf16 chunk in a 64B-swizzled 2 KB buffer
-// (conflict-free 16-byte st.shared) and one elected lane issues cp.async.bulk.tensor stores; residual chunks arrive
-// the same way in the other direction (per-warp mbarrier); the LayerNorm partial sums are kept SLOT-major
-// ([slot][row]) so that consecutive lanes touch consecutive addresses.
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-// 64B swizzle (CU_TENSOR_MAP_SWIZZLE_64B): 16-byte chunk index ^= address bits [7,9); rows of 64 bytes, 512-byte aligned buffer
-__device__ __forceinline__ uint32_t sw64_addr(uint32_t buf, int row, int piece) {
-  return buf + (uint32_t)row * 64u + ((uint32_t)(piece ^ ((row >> 1) & 3)) << 4);
-}
-
-// 256-bit global accesses (sm_100: STG/LDG.256): a thread's 64-byte bf16 row chunk leaves as two full 32-byte
-// sectors instead of four half-sector writes (which doubled the L1->L2 crossbar write traffic).
-__device__ __forceinline__ void st_global_256(void* p, const uint32_t (&r)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-__device__ __forceinline__ void ld_global_256(const void* p, uint4& lo, uint4& hi) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w), "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w) : "l"(p));
-}
-__device__ __forceinline__ void epi_store_packed(bf16* dst, const uint32_t (&pk)[16], bool wide) {
-  if (wide) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      uint32_t r[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) r[j] = pk[8 * i + j];
-      st_global_256(dst + 16 * i, r);
-    }
-    return;
-  }
-  uint4* d4 = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) d4[i] = make_uint4(pk[4 * i], pk[4 * i + 1], pk[4 * i + 2], pk[4 * i + 3]);
-}
-__device__ __forceinline__ void epi_store_bf16(bf16* dst, const float (&v)[32], bool wide) {
-  uint32_t pk[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) pk[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-  epi_store_packed(dst, pk, wide);
-}
-__device__ __forceinline__ void load_res_chunk(const bf16* src, uint4 (&r)[4], bool wide) {
-  if (wide) {
-    ld_global_256(src, r[0], r[1]);
-    ld_global_256(src + 16, r[2], r[3]);
-  } else {
-    const uint4* r4 = reinterpret_cast<const uint4*>(src);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) r[i] = __ldg(r4 + i);
-  }
-}
-
-// ---- epilogue of one 128-row x BN accumulator for the calling warp ------------------------------------------------
-// 16 epilogue warps: warp -> (TMEM lane quarter q = warp & 3, column group grp = 0..3); a warp handles the 32-column
-// chunks c = grp, grp + 4, ... of the tile, each as two 16-column halves (register budget: 640 threads x <= 102 regs).
-// Twice the warps per scheduler of the 8-warp layout: ncu showed the 8 warps latency-bound (8 cycles per issued
-// instruction, ~650 instructions per chunk, issue slots 30 % busy) and the short-K GEMMs bound by exactly that.
-struct EpiWarp {              // per-warp epilogue staging state (single-buffered: a warp owns <= 2 chunks per tile)
-  uint32_t out_stage;         // 2 KB: [32 rows][64 B], 64B-swizzled
-  uint32_t res_stage;         // 2 KB
-  uint32_t res_bar;           // mbarrier of the residual TMA load
-  uint32_t res_phase;
-};
-
-__device__ __forceinline__ void epi_res_issue(const CUtensorMap* tmRes, EpiWarp& ew, int lane, int row0, int col0) {
-  if (lane == 0) {
-    mbar_arrive_expect_tx(ew.res_bar, 2048);
-    tma_load_2d(ew.res_stage, tmRes, ew.res_bar, col0, row0);
-  }
-}
-// 8 bf16 pairs (columns [16 h, 16 h + 16) of this lane's row) of the staged residual chunk
-__device__ __forceinline__ void epi_res_half(const EpiWarp& ew, int lane, int h, uint4 (&r)[2]) {
-#pragma unroll
-  for (int j = 0; j < 2; ++j)
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r[j].x), "=r"(r[j].y), "=r"(r[j].z), "=r"(r[j].w)
-                 : "r"(sw64_addr(ew.res_stage, lane, 2 * h + j)) : "memory");
-}
-__device__ __forceinline__ void epi_stage_half(const EpiWarp& ew, int lane, int h, const uint32_t (&pk)[8]) {
-#pragma unroll
-  for (int j = 0; j < 2; ++j)
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sw64_addr(ew.out_stage, lane, 2 * h + j)), "r"(pk[4 * j]), "r"(pk[4 * j + 1]),
-                 "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3]) : "memory");
-}
-__device__ __forceinline__ void epi_tma_store(const GemmKParams& p, const CUtensorMap* tmOut, const EpiWarp& ew, int lane, int row0, int col0) {
-  fence_proxy_async();                                // generic-proxy writes -> visible to the TMA (async proxy)
-  __syncwarp();
-  if (lane == 0) {
-    if (p.tma_out == 3) tma_store_3d(tmOut, ew.out_stage, col0, row0 % p.orpb, row0 / p.orpb);
-    else tma_store_2d(tmOut, ew.out_stage, col0, row0);
-    tma_store_commit();
-  }
-}
-__device__ __forceinline__ void add4(float (&v)[16], int j, const float4 t) { v[j] += t.x; v[j + 1] += t.y; v[j + 2] += t.z; v[j + 3] += t.w; }
-
+// ---- epilogue of one 64-row x BN accumulator held by a consumer warpgroup ---------------------------------------
+// wgmma m64nN D fragment: warp w of the warpgroup holds rows 16 w + lane / 4 (regs 4 j + 0, 1) and + 8 (regs 4 j + 2, 3),
+// columns 8 j + 2 (lane % 4) + {0, 1}, for j = 0 .. N / 8 - 1.
 template <int BN, bool GEGLU>
-__device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t taddr, int row, int n_blk, int c0, float gate,
-                                              float ln_mu, float ln_rstd, const CUtensorMap* tmOut, const CUtensorMap* tmRes,
-                                              EpiWarp& ew, int lane) {
-  const bool row_ok = row < p.M;
-  const int row0 = row - lane;                        // first row of this warp's 32-row slab
-  const size_t out_off = p.orpb ? (size_t)(row / p.orpb) * p.obs + (size_t)(row % p.orpb) * p.ldc : (size_t)row * p.ldc;
-  constexpr int WOUT = GEGLU ? BN / 2 : BN;           // output columns of the tile
-  constexpr int NCH = WOUT / 32;
-  const bool tma_res = !GEGLU && p.tma_res;
-  const bool has_res = !GEGLU && p.residual != nullptr;
-  const float* rb = (!GEGLU && p.rowbias && row_ok) ? p.rowbias + (size_t)(row / p.rows_per_batch) * p.ld_rowbias : nullptr;
-#pragma unroll 1
-  for (int c = c0; c < NCH; c += 4) {
-    const int ocol = n_blk * WOUT + c * 32;           // first output column of the chunk
-    if (tma_res) {                                    // requested at the tile prologue (first chunk) or one chunk ago
-      mbar_wait(ew.res_bar, ew.res_phase);
-      ew.res_phase ^= 1u;
+__device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float (&d)[BN / 2], int row_base, int n_blk, float gate, int lane) {
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = row_base + hr * 8;
+    const bool row_ok = row < p.M;
+    float ln_mu = 0.f, ln_rstd = 1.f;
+    if (p.ln_stats && row_ok) {
+      const float2* sp = reinterpret_cast<const float2*>(p.ln_stats) + row;
+      float s1 = 0.f, s2 = 0.f;
+      for (int i = 0; i < p.ln_slots; ++i) { const float2 t = __ldg(sp + (size_t)i * p.ln_stride); s1 += t.x; s2 += t.y; }   // fixed order
+      ln_mu = s1 * p.inv_k;
+      ln_rstd = rsqrtf(fmaxf(s2 * p.inv_k - ln_mu * ln_mu, 0.f) + p.ln_eps);
     }
-    if (p.tma_out) {                                  // the staging buffer of this warp's previous chunk has been read out
-      if (lane == 0) tma_store_wait_read<0>();
-      __syncwarp();
-    }
-    float st_sum = 0.f, st_sq = 0.f;
+    const float c1 = -ln_rstd * ln_mu;              // LayerNorm fold: rstd * acc + (bias - rstd * mu * colsum)
+    const size_t out_off = p.orpb ? (size_t)(row / p.orpb) * p.obs + (size_t)(row % p.orpb) * p.ldc : (size_t)row * p.ldc;
+    if constexpr (GEGLU) {
+      constexpr int HALF = BN / 2;                  // packed weight rows per tile: [128 x | 128 gate]
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float v[16];
-      if constexpr (GEGLU) {
-        constexpr int HALF = BN / 2;
-        uint32_t rx[16], rg[16];
-        tmem_ld16(taddr + c * 32 + h * 16, rx);
-        tmem_ld16(taddr + HALF + c * 32 + h * 16, rg);
-        tmem_ld_wait();
-        const int wcol = n_blk * BN + c * 32 + h * 16;          // packed weight row of the x half ([128 x | 128 gate] per tile)
-        float g[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { v[j] = __uint_as_float(rx[j]); g[j] = __uint_as_float(rg[j]); }
-        // LayerNorm fold + bias as two FMAs per accumulator: rstd * acc + (bias - rstd * mu * colsum)
-        const float c1 = -ln_rstd * ln_mu;              // ln_rstd = 1, ln_mu = 0 without a fold
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float4 tx = __ldg(reinterpret_cast<const float4*>(p.bias + wcol + j));
-          float4 tg = __ldg(reinterpret_cast<const float4*>(p.bias + wcol + HALF + j));
-          if (p.ln_stats) {
-            const float4 ux = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + wcol + j));
-            const float4 ug = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + wcol + HALF + j));
-            tx.x = fmaf(ux.x, c1, tx.x); tx.y = fmaf(ux.y, c1, tx.y); tx.z = fmaf(ux.z, c1, tx.z); tx.w = fmaf(ux.w, c1, tx.w);
-            tg.x = fmaf(ug.x, c1, tg.x); tg.y = fmaf(ug.y, c1, tg.y); tg.z = fmaf(ug.z, c1, tg.z); tg.w = fmaf(ug.w, c1, tg.w);
-          }
-          v[j] = geglu_f(fmaf(v[j], ln_rstd, tx.x), fmaf(g[j], ln_rstd, tg.x));
-          v[j + 1] = geglu_f(fmaf(v[j + 1], ln_rstd, tx.y), fmaf(g[j + 1], ln_rstd, tg.y));
-          v[j + 2] = geglu_f(fmaf(v[j + 2], ln_rstd, tx.z), fmaf(g[j + 2], ln_rstd, tg.z));
-          v[j + 3] = geglu_f(fmaf(v[j + 3], ln_rstd, tx.w), fmaf(g[j + 3], ln_rstd, tg.w));
-        }
-      } else {
-        uint32_t r[16];
-        tmem_ld16(taddr + c * 32 + h * 16, r);
-        uint4 res[2] = {};
-        if (has_res) {
-          if (tma_res) epi_res_half(ew, lane, h, res);
-          else if (row_ok) {
-            const uint4* r4 = reinterpret_cast<const uint4*>(p.residual + (size_t)row * p.ldr + ocol + h * 16);
-            res[0] = __ldg(r4); res[1] = __ldg(r4 + 1);
-          }
-        }
-        tmem_ld_wait();
-        const int n0 = ocol + h * 16;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
+      for (int j = 0; j < HALF / 8; ++j) {
+        const int c = 8 * j + cq;
+        const int wcol = n_blk * BN + c;
+        float bx0 = __ldg(p.bias + wcol), bx1 = __ldg(p.bias + wcol + 1);
+        float bg0 = __ldg(p.bias + wcol + HALF), bg1 = __ldg(p.bias + wcol + HALF + 1);
         if (p.ln_stats) {
-          // LayerNorm fold + bias as two FMAs per element: rstd * acc + (bias - rstd * mu * colsum)
-          const float c1 = -ln_rstd * ln_mu;
+          bx0 = fmaf(__ldg(p.ln_colsum + wcol), c1, bx0); bx1 = fmaf(__ldg(p.ln_colsum + wcol + 1), c1, bx1);
+          bg0 = fmaf(__ldg(p.ln_colsum + wcol + HALF), c1, bg0); bg1 = fmaf(__ldg(p.ln_colsum + wcol + HALF + 1), c1, bg1);
+        }
+        const float x0 = fmaf(d[4 * j + 2 * hr], ln_rstd, bx0), x1 = fmaf(d[4 * j + 2 * hr + 1], ln_rstd, bx1);
+        const float g0 = fmaf(d[HALF / 2 + 4 * j + 2 * hr], ln_rstd, bg0), g1 = fmaf(d[HALF / 2 + 4 * j + 2 * hr + 1], ln_rstd, bg1);
+        if (row_ok)
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + out_off + n_blk * HALF + c) = pack_bf16x2(geglu_f(x0, g0), geglu_f(x1, g1));
+      }
+    } else {
+      const float* rb = (p.rowbias && row_ok) ? p.rowbias + (size_t)(row / p.rows_per_batch) * p.ld_rowbias : nullptr;
 #pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(p.ln_colsum + n0 + j));
-            float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias) bb = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + j));
-            v[j] = fmaf(v[j], ln_rstd, fmaf(t.x, c1, bb.x)); v[j + 1] = fmaf(v[j + 1], ln_rstd, fmaf(t.y, c1, bb.y));
-            v[j + 2] = fmaf(v[j + 2], ln_rstd, fmaf(t.z, c1, bb.z)); v[j + 3] = fmaf(v[j + 3], ln_rstd, fmaf(t.w, c1, bb.w));
+      for (int ch = 0; ch < BN / 32; ++ch) {        // 32-column chunks: one LayerNorm-statistics slot each
+        float st_sum = 0.f, st_sq = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * ch + jj;
+          const int n0 = n_blk * BN + 8 * j + cq;
+          float v0 = d[4 * j + 2 * hr], v1 = d[4 * j + 2 * hr + 1];
+          if (p.ln_stats) {
+            float b0 = 0.f, b1 = 0.f;
+            if (p.bias) { b0 = __ldg(p.bias + n0); b1 = __ldg(p.bias + n0 + 1); }
+            v0 = fmaf(v0, ln_rstd, fmaf(__ldg(p.ln_colsum + n0), c1, b0));
+            v1 = fmaf(v1, ln_rstd, fmaf(__ldg(p.ln_colsum + n0 + 1), c1, b1));
+          } else if (p.bias) add2(v0, v1, p.bias + n0);
+          if (rb) add2(v0, v1, rb + n0);
+          v0 = act_f(p.act, v0); v1 = act_f(p.act, v1);
+          if (p.gate) { v0 *= gate; v1 *= gate; }
+          if (p.residual && row_ok) {
+            const float2 r = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(p.residual + (size_t)row * p.ldr + n0)));
+            v0 += r.x; v1 += r.y;
           }
-        } else if (p.bias) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) add4(v, j, __ldg(reinterpret_cast<const float4*>(p.bias + n0 + j)));
-        }
-        if (rb) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) add4(v, j, __ldg(reinterpret_cast<const float4*>(rb + n0 + j)));
-        }
-        if (p.act == GLG_ACT_SILU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = silu_f(v[j]);
-        } else if (p.act == GLG_ACT_GELU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = gelu_erf_f(v[j]);
-        } else if (p.act == GLG_ACT_QUICK_GELU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = quick_gelu_f(v[j]);
-        }
-        if (p.gate) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] *= gate;
-        }
-        if (has_res) {
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            float2 f;
-            f = unpack_bf16x2(res[i].x); v[8 * i + 0] += f.x; v[8 * i + 1] += f.y;
-            f = unpack_bf16x2(res[i].y); v[8 * i + 2] += f.x; v[8 * i + 3] += f.y;
-            f = unpack_bf16x2(res[i].z); v[8 * i + 4] += f.x; v[8 * i + 5] += f.y;
-            f = unpack_bf16x2(res[i].w); v[8 * i + 6] += f.x; v[8 * i + 7] += f.y;
+          if (p.out_fp32) {
+            if (row_ok) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + out_off + n0) = make_float2(v0, v1);
+          } else {
+            const uint32_t pk = pack_bf16x2(v0, v1);
+            if (row_ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + out_off + n0) = pk;
+            // statistics of the values AS STORED (bf16-rounded): exactly what the consumer GEMM reads
+            const float2 f = unpack_bf16x2(pk);
+            st_sum += f.x + f.y;
+            st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
           }
         }
-        if (p.out_fp32) {
-          if (row_ok) {
-            float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + out_off + n0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) o4[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          }
-          continue;
+        if (p.stats_out && !p.out_fp32) {
+          // one partial per 32-column chunk, slot = global chunk index: independent of the tile shape, so the consumer's
+          // fixed-order sum is bit-identical whatever tile width produced the rows.  The four lanes of a row reduce in
+          // a fixed butterfly order.
+          st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 1); st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 1);
+          st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 2); st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 2);
+          if ((lane & 3) == 0 && row_ok)
+            reinterpret_cast<float2*>(p.stats_out)[(size_t)((n_blk * BN >> 5) + ch) * p.stats_stride + row] = make_float2(st_sum, st_sq);
         }
       }
-      uint32_t pk[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) pk[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-      if (!GEGLU && p.stats_out) {
-        // statistics of the values AS STORED (bf16-rounded): exactly what the consumer GEMM reads
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 f = unpack_bf16x2(pk[j]);
-          st_sum += f.x + f.y;
-          st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
-        }
-      }
-      if (p.tma_out) epi_stage_half(ew, lane, h, pk);
-      else if (row_ok) {
-        uint4* d4 = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(p.out) + out_off + ocol + h * 16);
-        d4[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        d4[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-      }
     }
-    if (tma_res) {
-      __syncwarp();                                   // every lane holds its residual values: the buffer may be refilled
-      if (c + 4 < NCH) epi_res_issue(tmRes, ew, lane, row0, ocol + 128);
-    }
-    if (!GEGLU && p.stats_out && row_ok && !p.out_fp32) {
-      // one partial per 32-column chunk, slot = global chunk index: independent of the tile shape, so the consumer's
-      // fixed-order sum is bit-identical whatever kernel variant produced the rows.  SLOT-major: the 32 lanes
-      // (consecutive rows) write 256 consecutive bytes.
-      reinterpret_cast<float2*>(p.stats_out)[(size_t)(ocol >> 5) * p.stats_stride + row] = make_float2(st_sum, st_sq);
-    }
-    if (p.tma_out && !(p.dbg & 8)) epi_tma_store(p, tmOut, ew, lane, row0, ocol);
   }
 }
 
 // split-K: raw fp32 accumulators -> ws[split][row][n]
 template <int BN>
-__device__ __forceinline__ void epilogue_partial(const GemmKParams& p, uint32_t taddr, int row, int n_blk, int c0, int split) {
-  constexpr int NCH = BN / 32;
-  float* dst = p.ws + ((size_t)split * p.M + row) * p.N + (size_t)n_blk * BN;
-#pragma unroll 1
-  for (int c = c0; c < NCH; c += 4) {
+__device__ __forceinline__ void epilogue_partial(const GemmKParams& p, const float (&d)[BN / 2], int row_base, int n_blk, int split, int lane) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t r[16];
-      tmem_ld16(taddr + c * 32 + h * 16, r);
-      tmem_ld_wait();
-      if (row < p.M) {
-        float4* o4 = reinterpret_cast<float4*>(dst + c * 32 + h * 16);
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = row_base + hr * 8;
+    if (row >= p.M) continue;
+    float* dst = p.ws + ((size_t)split * p.M + row) * p.N + (size_t)n_blk * BN + 2 * (lane & 3);
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          o4[i] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3]));
-      }
-    }
+    for (int j = 0; j < BN / 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(d[4 * j + 2 * hr], d[4 * j + 2 * hr + 1]);
   }
 }
 
@@ -456,16 +209,8 @@ __global__ void splitk_reduce_kernel(const GemmKParams p) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] += __ldg(rb + j);
     }
-    if (p.act == GLG_ACT_SILU) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = silu_f(v[j]);
-    } else if (p.act == GLG_ACT_GELU) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = gelu_erf_f(v[j]);
-    } else if (p.act == GLG_ACT_QUICK_GELU) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = quick_gelu_f(v[j]);
-    }
+    for (int j = 0; j < 8; ++j) v[j] = act_f(p.act, v[j]);
     if (p.gate) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] *= gate;
@@ -486,9 +231,8 @@ __global__ void splitk_reduce_kernel(const GemmKParams p) {
 }
 
 template <int BN, bool GEGLU, bool CTA2>
-__global__ void __launch_bounds__(640, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes, const GemmKParams p) {
+__global__ void __launch_bounds__(384, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
   using Cfg = GemmCfg<BN, CTA2>;
   constexpr int MAXST = Cfg::MAX_STAGES;
   constexpr int ROWS_PER_TILE = CTA2 ? 256 : 128;
@@ -501,43 +245,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t bres_base = base + (uint32_t)STAGES * Cfg::A_BYTES;  // resident weight tile: num_kb x [BN rows x 128 B]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (MAXST + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * MAXST + a); };
-  constexpr int ACC = Cfg::ACC;
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * MAXST + ACC + a); };
-  const uint32_t bfull_bar = bar_base + 8u * (2 * MAXST + 2 * ACC);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * MAXST + 2 * ACC + 1);
-  const uint32_t res_bars = bar_base + 8u * (2 * MAXST + 2 * ACC + 2);      // 16 epilogue warps
+  const uint32_t bfull_bar = bar_base + 8u * (2 * MAXST);
 
   pdl_trigger();          // the next kernel may start its prologue while this one runs (it waits before touching memory)
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = CTA2 ? cluster_ctarank() : 0u;       // 0 = leader (issues the MMAs)
+  const int wg = warp >> 2;
+  const uint32_t rank = CTA2 ? cluster_ctarank() : 0u;
   const int unit = CTA2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;          // CTA or CTA-pair index
   const int num_units = CTA2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
+  if (threadIdx.x == 0) {
+    // a stage is free again when every consumer warp (8 per CTA) of every CTA that receives it has released it
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CTA2 ? 16 : 8); }
     mbar_init(bfull_bar, 1);
-    for (int i = 0; i < 16; ++i) mbar_init(res_bars + 8u * i, 1);          // one per epilogue warp
-    // accumulator drained: one arrive per epilogue warp (16), from both CTAs of a pair (on the leader's barrier)
-    for (int a = 0; a < ACC; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), CTA2 ? 32 : 16); }
     fence_barrier_init();
   }
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-      if (p.tma_out) tma_prefetch_desc(&tmOut);
-      if (p.tma_res) tma_prefetch_desc(&tmRes);
-    }
-    __syncwarp();
-    if constexpr (CTA2) { tmem_alloc2(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish2(); }
-    else { tmem_alloc(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
+  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); }
   if constexpr (CTA2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
   pdl_wait();             // everything above overlapped the previous kernel's tail; global data is touched only below
 
   const int total_work = p.tiles_m * p.tiles_n * p.splits;
@@ -559,165 +284,114 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     return true;
   };
 
-  if (warp == 0) {
-    // ===================== TMA producer (every CTA loads its own 128 rows of A and its share of B) ==========
-    // whole warp walks the loop, one elected lane issues (see elect_one())
-    const bool leader = elect_one();
-    int stage = 0; uint32_t phase = 0;
-    if (bres && leader) {
-      // the CTA's weight tile, once: num_kb boxes of [BN rows x 64 columns] on one barrier
-      const int brow = (unit % p.tiles_n) * BN;
-      mbar_arrive_expect_tx(bfull_bar, (uint32_t)p.num_kb * Cfg::B_BYTES);
-      for (int kb = 0; kb < p.num_kb; ++kb) tma_load_2d(bres_base + (uint32_t)kb * Cfg::B_BYTES, &tmB, bfull_bar, kb * 64, brow);
-    }
-    int tile, split, m_blk, n_blk;
-    for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
-      const int kb_lo = (split * p.num_kb) / p.splits, kb_n = ((split + 1) * p.num_kb) / p.splits - kb_lo;
-      const int row0 = m_blk * ROWS_PER_TILE + (int)rank * 128;
-      int b0 = 0, y0 = 0, x0 = 0;
-      if (p.conv) {
-        b0 = row0 / p.HW;
-        y0 = (row0 - b0 * p.HW) / p.Wd;
-        x0 = row0 - b0 * p.HW - y0 * p.Wd;          // non-zero only for images wider than a tile (W > 128: part of one row)
+  if (wg == 0) {
+    setmaxnreg_dec40();
+    if (warp == 0) {
+      // ===================== TMA producer: whole warp walks the loop, one elected lane issues =====================
+      const bool leader = elect_one();
+      int stage = 0; uint32_t phase = 0;
+      if (bres && leader) {
+        // the CTA's weight tile, once: num_kb boxes of [BN rows x 64 columns] on one barrier
+        const int brow = (unit % p.tiles_n) * BN;
+        mbar_arrive_expect_tx(bfull_bar, (uint32_t)p.num_kb * Cfg::B_BYTES);
+        for (int kb = 0; kb < p.num_kb; ++kb) tma_load_2d(bres_base + (uint32_t)kb * Cfg::B_BYTES, &tmB, bfull_bar, kb * 64, brow);
       }
-      const int brow0 = n_blk * BN + (int)rank * Cfg::BROWS;
-      // K steps are visited in a per-tile rotated order: tiles running at the same time would otherwise request
-      // the very same weight (and activation) lines from L2 in lockstep; the rotation spreads them over slices.
-      // (fp32 accumulation order depends only on the tile index -> results stay reproducible.)  B-resident tiles
-      // fetch no weights per tile and walk K in order (the MMA warp indexes the resident tile by K step).
-      int kb = bres ? kb_lo : kb_lo + (int)(((unsigned)tile * 3u) % (unsigned)kb_n);
-      for (int it2 = 0; it2 < kb_n; ++it2, kb = (kb + 1 == kb_lo + kb_n) ? kb_lo : kb + 1) {
-        mbar_wait(empty_bar(stage), phase ^ 1u);
-        const uint32_t a_dst = base + stage * stage_bytes;
-        const uint32_t b_dst = a_dst + Cfg::A_BYTES;
-        if (leader && (p.dbg & 1)) {
-          if (!CTA2 || rank == 0) mbar_arrive(full_bar(stage));
-        } else if (leader) {
-        // the leader CTA's barrier collects the bytes of both CTAs
-        if (bres) mbar_arrive_expect_tx(full_bar(stage), Cfg::A_BYTES);
-        else if (!CTA2) mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-        else if (rank == 0) mbar_arrive_expect_tx(full_bar(stage), 2 * Cfg::STAGE_BYTES);
+      int tile, split, m_blk, n_blk;
+      for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
+        const int kb_lo = (split * p.num_kb) / p.splits, kb_n = ((split + 1) * p.num_kb) / p.splits - kb_lo;
+        const int row0 = m_blk * ROWS_PER_TILE + (int)rank * 128;
+        int b0 = 0, y0 = 0, x0 = 0;
         if (p.conv) {
-          const int tap = kb / p.kb_per_tap;
-          const int cb = kb - tap * p.kb_per_tap;
-          const int dy = tap / 3 - 1, dx = tap - (tap / 3) * 3 - 1;
-          if constexpr (CTA2) {
-            tma_load_4d_2sm(a_dst, &tmA, full_bar(stage), cb * 64, x0 + dx, y0 + dy, b0);
-            tma_load_2d_2sm(b_dst, &tmB, full_bar(stage), cb * 64, tap * p.N + brow0);
-          } else {
-            tma_load_4d(a_dst, &tmA, full_bar(stage), cb * 64, x0 + dx, y0 + dy, b0);
-            tma_load_2d(b_dst, &tmB, full_bar(stage), cb * 64, tap * p.N + brow0);
-          }
-        } else {
-          if constexpr (CTA2) {
-            tma_load_2d_2sm(a_dst, &tmA, full_bar(stage), kb * 64, row0);
-            tma_load_2d_2sm(b_dst, &tmB, full_bar(stage), kb * 64, brow0);
-          } else {
-            tma_load_2d(a_dst, &tmA, full_bar(stage), kb * 64, row0);
-            if (!bres) tma_load_2d(b_dst, &tmB, full_bar(stage), kb * 64, brow0);
-          }
+          b0 = row0 / p.HW;
+          y0 = (row0 - b0 * p.HW) / p.Wd;
+          x0 = row0 - b0 * p.HW - y0 * p.Wd;          // non-zero only for images wider than a tile (W > 128: part of one row)
         }
+        const int brow0 = n_blk * BN;
+        // K steps are visited in a per-tile rotated order: tiles running at the same time would otherwise request
+        // the very same weight (and activation) lines from L2 in lockstep; the rotation spreads them over slices.
+        // (fp32 accumulation order depends only on the tile index -> results stay reproducible.)  B-resident tiles
+        // fetch no weights per tile and walk K in order (the consumers index the resident tile by K step).
+        int kb = bres ? kb_lo : kb_lo + (int)(((unsigned)tile * 3u) % (unsigned)kb_n);
+        for (int it2 = 0; it2 < kb_n; ++it2, kb = (kb + 1 == kb_lo + kb_n) ? kb_lo : kb + 1) {
+          mbar_wait<false>(empty_bar(stage), phase ^ 1u);
+          const uint32_t a_dst = base + stage * stage_bytes;
+          const uint32_t b_dst = a_dst + Cfg::A_BYTES;
+          if (leader) {
+            mbar_arrive_expect_tx(full_bar(stage), bres ? Cfg::A_BYTES : Cfg::STAGE_BYTES);
+            int ca = kb * 64, cb_row = brow0;
+            if (p.conv) {
+              const int tap = kb / p.kb_per_tap;
+              const int cb = kb - tap * p.kb_per_tap;
+              const int dy = tap / 3 - 1, dx = tap - (tap / 3) * 3 - 1;
+              tma_load_4d(a_dst, &tmA, full_bar(stage), cb * 64, x0 + dx, y0 + dy, b0);
+              ca = cb * 64; cb_row = tap * p.N + brow0;
+            } else {
+              tma_load_2d(a_dst, &tmA, full_bar(stage), kb * 64, row0);
+            }
+            if constexpr (CTA2) {
+              tma_load_2d_mc(b_dst + rank * Cfg::B_HALF, &tmB, full_bar(stage), ca, cb_row + (int)rank * (BN / 2), (uint16_t)3);
+            } else if (!bres) {
+              tma_load_2d(b_dst, &tmB, full_bar(stage), ca, cb_row);
+            }
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1 && rank == 0) {
-    // ===================== MMA issuer (leader CTA only; one elected lane issues, see elect_one()) =====================
-    constexpr uint32_t idesc = umma_idesc_bf16(CTA2 ? 256 : 128, BN);
-    const bool leader = elect_one();
+  } else {
+    // ===================== consumers: warpgroup 1 / 2 own accumulator rows [0, 64) / [64, 128) of the tile ==========
+    setmaxnreg_inc232();
+    const int cw = wg - 1;
+    const float gate = p.gate ? __ldg(p.gate) : 1.0f;
+    uint32_t empty0 = empty_bar(0), empty0_peer = 0;
+    if constexpr (CTA2) empty0_peer = mapa_cluster(empty_bar(0), rank ^ 1u);
+    if (bres) mbar_wait<false>(bfull_bar, 0);
     int stage = 0; uint32_t phase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
-    if (bres) { mbar_wait(bfull_bar, 0); tc_fence_after(); }
+    auto release = [&](int s) {
+      if (lane == 0) {
+        mbar_arrive(empty0 + 8u * s);
+        if constexpr (CTA2) mbar_arrive_cluster(empty0_peer + 8u * s);
+      }
+    };
+    float d[BN / 2];
     int tile, split, m_blk, n_blk;
     for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
       const int kb_n = ((split + 1) * p.num_kb) / p.splits - (split * p.num_kb) / p.splits;
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
+      int prev = -1;
       for (int kb = 0; kb < kb_n; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint32_t a_addr = base + stage * stage_bytes;
-        const uint64_t adesc = umma_desc_kmajor_sw128(a_addr);
-        const uint64_t bdesc = umma_desc_kmajor_sw128(bres ? bres_base + (uint32_t)kb * Cfg::B_BYTES : a_addr + Cfg::A_BYTES);
-        if (leader) {
-          if (!(p.dbg & 2))
+        mbar_wait<false>(full_bar(stage), phase);
+        const uint32_t a_addr = base + stage * stage_bytes + (uint32_t)cw * (64 * 128);
+        const uint64_t adesc = gmma_desc_kmajor_sw128(a_addr);
+        const uint64_t bdesc = gmma_desc_kmajor_sw128(bres ? bres_base + (uint32_t)kb * Cfg::B_BYTES : base + stage * stage_bytes + Cfg::A_BYTES);
+        wgmma_fence_regs(d);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {   // 4 x K=16 inside one 64-wide (128 B) swizzle atom: +32 B per step
-            if constexpr (CTA2) umma_bf16_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            else umma_bf16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          if constexpr (CTA2) umma_commit_2sm(empty_bar(stage)); else umma_commit(empty_bar(stage));
-        }
+        for (int k = 0; k < 4; ++k)      // 4 x K=16 inside one 64-wide (128 B) swizzle atom: +32 B per step
+          Wgmma<BN>::mma(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its buffers back to the producer
+        wgmma_fence_regs(d);
+        if (prev >= 0) release(prev);
+        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
-      if (leader) {
-        if constexpr (CTA2) umma_commit_2sm(tfull_bar(acc)); else umma_commit(tfull_bar(acc));
-      }
-      if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      if (prev >= 0) release(prev);
+      const int row_base = m_blk * ROWS_PER_TILE + (int)rank * 128 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+      if (p.splits > 1) epilogue_partial<BN>(p, d, row_base, n_blk, split, lane);
+      else epilogue_tile<BN, GEGLU>(p, d, row_base, n_blk, gate, lane);
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue (each CTA: its own 128 accumulator rows; 16 warps) =====================
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int grp = (warp - 4) >> 2;              // column group: chunks grp, grp + 4, ...
-    int acc = 0; uint32_t acc_phase = 0;
-    const float gate = p.gate ? __ldg(p.gate) : 1.0f;
-    const uint32_t tempty_leader0 = CTA2 ? mapa_cluster(tempty_bar(0), 0) : tempty_bar(0);   // consecutive stages: +8 bytes
-    EpiWarp ew;
-    ew.out_stage = base + p.epi_off + (uint32_t)(warp - 4) * 2048u;
-    ew.res_stage = base + p.epi_off + 32768u + (uint32_t)(warp - 4) * 2048u;
-    ew.res_bar = res_bars + 8u * (uint32_t)(warp - 4);
-    ew.res_phase = 0;
-    constexpr int NCH_OUT = (GEGLU ? BN / 2 : BN) / 32;
-    int tile, split, m_blk, n_blk;
-    for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
-      const int row = m_blk * ROWS_PER_TILE + (int)rank * 128 + q * 32 + lane;
-      // ---- prefetch what does not depend on the accumulator: LayerNorm statistics and the first residual chunk
-      float ln_mu = 0.f, ln_rstd = 1.f;
-      if (p.ln_stats && row < p.M) {
-        const float2* sp = reinterpret_cast<const float2*>(p.ln_stats) + row;          // slot-major: coalesced across the warp
-        float s1 = 0.f, s2 = 0.f;
-        for (int i = 0; i < p.ln_slots; ++i) { const float2 t = __ldg(sp + (size_t)i * p.ln_stride); s1 += t.x; s2 += t.y; }   // fixed order
-        ln_mu = s1 * p.inv_k;
-        ln_rstd = rsqrtf(fmaxf(s2 * p.inv_k - ln_mu * ln_mu, 0.f) + p.ln_eps);
-      }
-      // chunk -> column group rotates with the tile counter: with 5 chunks per tile (BN = 160) group 0 would otherwise
-      // own two chunks of EVERY tile and set the pace; over four tiles every group now handles five
-      const int c0 = (grp - it) & 3;
-      if (!GEGLU && p.tma_res && p.splits == 1 && !(p.dbg & 4) && c0 < NCH_OUT)
-        epi_res_issue(&tmRes, ew, lane, row - lane, n_blk * BN + c0 * 32);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN;
-      if (p.dbg & 4) {
-      } else if (p.splits > 1) epilogue_partial<BN>(p, taddr, row, n_blk, c0, split);
-      else epilogue_tile<BN, GEGLU>(p, taddr, row, n_blk, c0, gate, ln_mu, ln_rstd, &tmOut, &tmRes, ew, lane);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        const uint32_t bar = tempty_leader0 + 8u * acc;
-        if constexpr (CTA2) mbar_arrive_cluster(bar); else mbar_arrive(bar);
-      }
-      if (++acc == ACC) { acc = 0; acc_phase ^= 1u; }
-    }
-    if (p.tma_out && lane == 0) tma_store_wait_read<0>();     // the staging buffers must outlive the TMA's reads
   }
-
-  tc_fence_before();
-  if constexpr (CTA2) cluster_sync_all(); else __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    tc_fence_after();
-    if constexpr (CTA2) tmem_dealloc2(tmem_base, Cfg::TMEM_COLS); else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+  // no CTA of a pair may exit while its peer can still multicast into its smem or arrive on its barriers
+  if constexpr (CTA2) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------
 // launch
 // ------------------------------------------------------------------------------------------------
 template <int BN, bool GEGLU, bool CTA2>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const CUtensorMap& tres, const GemmKParams& p,
-                       size_t smem, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, size_t smem, cudaStream_t st) {
   using Cfg = GemmCfg<BN, CTA2>;
   static bool attr_set = false;
   auto kern = gemm_tc_kernel<BN, GEGLU, CTA2>;
@@ -736,7 +410,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   } else {
     grid = tiles < num_sms() ? tiles : num_sms();
   }
-  cudaError_t e = launch_k(kern, dim3(grid), dim3(640), smem, st, CTA2 ? 2 : 1, ta, tb, tout, tres, p);
+  cudaError_t e = launch_k(kern, dim3(grid), dim3(Cfg::THREADS), smem, st, CTA2 ? 2 : 1, ta, tb, p);
   count_launch();
   if (e != cudaSuccess) return set_error(std::string("gemm launch: ") + cudaGetErrorString(e));
   if (check_launch("gemm launch")) return -1;
@@ -755,23 +429,22 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
 int g_force_bn = 0;     // test hooks (glg_debug_force_bn / glg_debug_gemm_cta2 / glg_debug_splitk)
 int g_splitk_mode = 0;  // 0 = heuristic, 1 = never, 2 = split whenever legal
 int g_cta2_mode = -1;   // 0 = heuristic, 1 = never pair, 2 = pair whenever legal; -1 = read GLG_GEMM_CTA2 (default 0)
-int g_gemm_dbg = 0;     // scripts/micro knock-out flags (GemmKParams::dbg)
-int g_epi_mode = -1;    // test hook: -1 = GLG_GEMM_EPI / default, 0 = per-thread epilogue accesses, 1 = TMA epilogue
-int g_bres_mode = -1;   // B-resident tiles: 0 = heuristic, 1 = never, 2 = whenever legal; -1 = read GLG_GEMM_BRES (default 0)
+int g_bres_mode = -1;   // B-resident tiles: 0 = heuristic, 1 = never, 2 = whenever legal; -1 = read GLG_GEMM_BRES (default 1)
+
+static constexpr long long kTileMax = 227 * 1024 - 1024 - 1024;     // dynamic smem minus alignment slack and barriers
 
 // A stages left beside a resident [BN x K] weight tile (0: does not fit)
 static int bres_stages(int bn, int num_kb) {
-  const long long tile_max = 227 * 1024 - 1024 - 1024;
-  const long long left = tile_max - (long long)num_kb * bn * 128;
+  const long long left = kTileMax - (long long)num_kb * bn * 128;
   if (left < 3 * 16384) return 0;
   const int st = (int)(left / 16384);
   return st > 12 ? 12 : st;
 }
 
-// Tile / split choice by a small time model (cycles):
-//   per 64-wide K step an SM needs max(MMA = 2*BN, operand bytes / ~42 B/clk of L2->SM bandwidth) cycles (a pair
-//   stages 128 + BN/2 operand rows per SM instead of 128 + BN); a CTA pays ~3000 cycles of fixed cost per work item;
-//   split-K adds a reduce pass over splits * M * N fp32.  The least estimated time wins.
+// Tile / split choice by a small time model (cycles, H100 data-sheet rates, not tuned by measurement):
+//   per 64-wide K step an SM needs max(MMA = 4*BN: 128 x BN x 64 MACs at 2048 bf16 MAC/clk, operand bytes / ~32 B/clk of
+//   L2->SM bandwidth) cycles (a pair stages 128 + BN/2 operand rows per SM instead of 128 + BN); a CTA pays ~3000 cycles
+//   of fixed cost per work item; split-K adds a reduce pass over splits * M * N fp32.  The least estimated time wins.
 static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_splits, long long ws_bytes,
                       int* bn_out, int* cta2_out, int* splits_out, int* bres_out) {
   if (g_cta2_mode < 0) {
@@ -780,15 +453,14 @@ static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_s
   }
   if (g_bres_mode < 0) {
     const char* e = getenv("GLG_GEMM_BRES");
-    g_bres_mode = e ? atoi(e) : 1;      // measured (profiles/r2): no gain while the epilogue bounds the short-K tiles -> opt-in
+    g_bres_mode = e ? atoi(e) : 1;      // opt-in
   }
   const int sms = num_sms();
   const int cands[4] = {256, 160, 128, 64};
   float best = 1e30f; int best_bn = 0, best_pair = 0, best_s = 1, best_res = 0;
   for (int pair = 0; pair < 2; ++pair) {
     if (pair && (g_cta2_mode == 1 || M <= 128)) continue;
-    // measured on B200 (profiles/): pairing pays for large, long-K, N % 256 == 0 GEMMs (M = 2048 pairs lose 20 %) and, by
-    // 3-10 %, for the 3x3 convolutions from 16x16 up at 2B = 8 (profiles/r2_kernels.txt); never for the split-K cases
+    // the heuristic pairs only large, long-K plain GEMMs with N % 256 == 0 and the larger 3x3 convolutions
     if (pair && g_cta2_mode == 0 && !conv && (N % 256 || num_kb < 16 || M < 4096)) continue;
     if (pair && g_cta2_mode == 0 && conv && M < 2048) continue;
     if (!pair && g_cta2_mode == 2 && M > 128) {
@@ -806,8 +478,8 @@ static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_s
       const int rows = pair ? 256 : 128;
       const int tiles = ((M + rows - 1) / rows) * (N / bn);
       const int units = pair ? sms / 2 : sms;
-      const float mma = 2.0f * bn;
-      const float l2 = 3.05f * (pair ? 128.0f + 0.5f * bn : 128.0f + bn);
+      const float mma = 4.0f * bn;
+      const float l2 = 4.0f * (pair ? 128.0f + 0.5f * bn : 128.0f + bn);
       const float per_kb = mma > l2 ? mma : l2;
       for (int sp = 1; sp <= (pair ? 1 : max_splits); ++sp) {
         if (sp > 1 && (num_kb / sp < (g_splitk_mode == 2 ? 4 : 16) || (long long)sp * M * N * 4 > ws_bytes)) break;
@@ -816,7 +488,7 @@ static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_s
         const int waves = (tiles * sp + units - 1) / units;
         const int kb_cta = (num_kb + sp - 1) / sp;
         float t = (float)waves * (per_kb * kb_cta + 3000.0f);
-        if (sp > 1) t += 12000.0f + (float)sp * M * N * 4.0f / (sms * 40.0f);     // slab round trip + reduce launch (sweep_bn)
+        if (sp > 1) t += 12000.0f + (float)sp * M * N * 4.0f / (sms * 40.0f);     // slab round trip + reduce launch
         const int ctas = (pair ? 2 : 1) * (tiles * sp < units ? tiles * sp : units);
         t *= 1.0f + 0.10f * (1.0f - (float)ctas / (float)sms);     // idle SMs: prefer the finer decomposition
         if (t < best) { best = t; best_bn = bn; best_pair = pair; best_s = sp; best_res = 0; }
@@ -827,8 +499,8 @@ static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_s
         const int per_n = sms / tiles_n;
         if (tiles_m >= 2 * per_n || g_bres_mode == 2) {
           const int waves = (tiles_m + per_n - 1) / per_n;
-          const float l2a = 3.05f * 128.0f;
-          float t = (float)waves * ((mma > l2a ? mma : l2a) * num_kb + 3000.0f) + 3.05f * bn * num_kb;
+          const float l2a = 4.0f * 128.0f;
+          float t = (float)waves * ((mma > l2a ? mma : l2a) * num_kb + 3000.0f) + 4.0f * bn * num_kb;
           const int ctas = per_n * tiles_n;
           t *= 1.0f + 0.10f * (1.0f - (float)ctas / (float)sms);
           if (g_bres_mode == 2) t = -1.0f / (float)bn;            // test hook: force (widest legal tile)
@@ -852,8 +524,6 @@ extern "C" void glg_debug_pick_tile(int M, int N, int K, int geglu, int conv, in
   out[1] |= bres << 8;           // bit 8 of the "paired" word: B-resident
 }
 extern "C" void glg_debug_gemm_bres(int mode) { glg::g_bres_mode = mode; }
-extern "C" void glg_debug_gemm_epi(int mode) { glg::g_epi_mode = mode; }
-extern "C" void glg_debug_gemm_knockout(int flags) { glg::g_gemm_dbg = flags; }
 extern "C" void glg_debug_gemm_cta2(int mode) { glg::g_cta2_mode = mode; }
 extern "C" void glg_debug_splitk(int mode) { glg::g_splitk_mode = mode; }
 
@@ -899,43 +569,21 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
     p.orpb = a->out_rows_per_batch; p.obs = a->out_batch_stride;
   }
   if (a->bias && ((uintptr_t)a->bias & 15)) return set_error("glg_gemm: bias must be 16-byte aligned");
-  p.wide = !a->out_fp32 && !((uintptr_t)a->out & 31) && !(a->ldc % 16) && !(a->out_batch_stride % 16) &&
-           (!a->residual || (!((uintptr_t)a->residual & 31) && !(a->ldr % 16)));
 
   p.splits = splits;
   p.ws = splits > 1 ? reinterpret_cast<float*>(a->splitk_ws) : nullptr;
   p.b_res = bres;
-  p.dbg = g_gemm_dbg;
-  // ---- epilogue data path: TMA stores of the bf16 output, TMA loads of the residual (see the kernel comment)
-  static int epi_mode = -1;       // GLG_GEMM_EPI: 0 = per-thread global accesses (the old path), 1 = TMA (default)
-  if (epi_mode < 0) { const char* e = getenv("GLG_GEMM_EPI"); epi_mode = e ? atoi(e) : 1; }
-  const int epi = g_epi_mode >= 0 ? g_epi_mode : epi_mode;
-  p.tma_out = 0; p.tma_res = 0;
-  if (epi && !a->out_fp32 && splits == 1) {
-    if (a->out_rows_per_batch <= 0) p.tma_out = 2;
-    else if (a->out_rows_per_batch % 32 == 0 && a->M % a->out_rows_per_batch == 0) p.tma_out = 3;
-  }
-  if (p.tma_out && a->residual && !a->geglu) p.tma_res = 1;
-  const long long tile_max = 227 * 1024 - 1024 - 1024;
-  const long long stage_bytes = bres ? 16384 : 128 * 128 + (cta2 ? bn / 2 : bn) * 128;
+  const long long stage_bytes = bres ? 16384 : 128 * 128 + bn * 128;
   const long long fixed = bres ? (long long)p.num_kb * bn * 128 : 0;
-  auto stages_for = [&](int out_on, int res_on) {
-    long long st = (tile_max - fixed - (out_on ? 32768 : 0) - (res_on ? 32768 : 0)) / stage_bytes;
-    const int cap = bres ? 12 : 8;
-    return (int)(st > cap ? cap : st);
-  };
-  // the staging area must not starve the operand ring: long-K tiles keep >= 4 stages (the residual staging goes first)
-  const int min_stages = p.num_kb >= 16 ? 4 : 3;
-  if (p.tma_res && stages_for(1, 1) < min_stages) p.tma_res = 0;
-  if (p.tma_out && stages_for(1, p.tma_res) < min_stages) { p.tma_out = 0; p.tma_res = 0; }
-  p.stages = stages_for(p.tma_out, p.tma_res);
+  long long stages = (kTileMax - fixed) / stage_bytes;
+  const int cap = bres ? 12 : 8;
+  p.stages = (int)(stages > cap ? cap : stages);
   if (p.stages < 2) return set_error("glg_gemm: internal: shared memory budget");
-  p.epi_off = (unsigned)(p.stages * stage_bytes + fixed);
-  const size_t smem = (size_t)p.epi_off + (p.tma_out ? 32768 : 0) + (p.tma_res ? 32768 : 0) + 1024 + 1024;
+  const size_t smem = (size_t)(p.stages * stage_bytes + fixed) + 1024 + 1024;
   if (a->stats_out) p.stats_stride = a->stats_slot_stride > 0 ? a->stats_slot_stride : a->M;
   if (a->ln_stats) p.ln_stride = a->ln_slot_stride > 0 ? a->ln_slot_stride : a->M;
 
-  const uint32_t brows = (uint32_t)(cta2 ? bn / 2 : bn);
+  const uint32_t brows = (uint32_t)(cta2 ? bn / 2 : bn);           // a pair: each CTA multicasts half of the B tile
   CUtensorMap ta, tb;
   if (a->conv_mode) {
     const int H = a->H, W = a->Wd, B = a->Bn;
@@ -970,41 +618,21 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
     const uint32_t wb[2] = {64, brows};
     if (get_tmap_bf16(&tb, a->W, 2, wd, ws, wb)) return -1;
   }
-  CUtensorMap tout = ta, tres = ta;          // placeholders when unused (never dereferenced by the kernel)
-  if (p.tma_out) {
-    const uint64_t No = a->geglu ? (uint64_t)a->N / 2 : (uint64_t)a->N;
-    const uint32_t box3[3] = {32, 32, 1};
-    if (p.tma_out == 2) {
-      const uint64_t dims[2] = {No, (uint64_t)a->M};
-      const uint64_t str[1] = {(uint64_t)a->ldc * 2};
-      if (get_tmap_bf16_sw(&tout, a->out, 2, dims, str, box3, 64)) return -1;
-    } else {
-      const uint64_t dims[3] = {No, (uint64_t)a->out_rows_per_batch, (uint64_t)(a->M / a->out_rows_per_batch)};
-      const uint64_t str[2] = {(uint64_t)a->ldc * 2, (uint64_t)a->out_batch_stride * 2};
-      if (get_tmap_bf16_sw(&tout, a->out, 3, dims, str, box3, 64)) return -1;
-    }
-  }
-  if (p.tma_res) {
-    const uint64_t dims[2] = {(uint64_t)a->N, (uint64_t)a->M};
-    const uint64_t str[1] = {(uint64_t)a->ldr * 2};
-    const uint32_t box2[2] = {32, 32};
-    if (get_tmap_bf16_sw(&tres, a->residual, 2, dims, str, box2, 64)) return -1;
-  }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (cta2) {
-    if (a->geglu) return launch_gemm<256, true, true>(ta, tb, tout, tres, p, smem, st);
+    if (a->geglu) return launch_gemm<256, true, true>(ta, tb, p, smem, st);
     switch (bn) {
-      case 256: return launch_gemm<256, false, true>(ta, tb, tout, tres, p, smem, st);
-      case 160: return launch_gemm<160, false, true>(ta, tb, tout, tres, p, smem, st);
-      case 128: return launch_gemm<128, false, true>(ta, tb, tout, tres, p, smem, st);
+      case 256: return launch_gemm<256, false, true>(ta, tb, p, smem, st);
+      case 160: return launch_gemm<160, false, true>(ta, tb, p, smem, st);
+      case 128: return launch_gemm<128, false, true>(ta, tb, p, smem, st);
     }
   } else {
-    if (a->geglu) return launch_gemm<256, true, false>(ta, tb, tout, tres, p, smem, st);
+    if (a->geglu) return launch_gemm<256, true, false>(ta, tb, p, smem, st);
     switch (bn) {
-      case 256: return launch_gemm<256, false, false>(ta, tb, tout, tres, p, smem, st);
-      case 160: return launch_gemm<160, false, false>(ta, tb, tout, tres, p, smem, st);
-      case 128: return launch_gemm<128, false, false>(ta, tb, tout, tres, p, smem, st);
-      case 64:  return launch_gemm<64, false, false>(ta, tb, tout, tres, p, smem, st);
+      case 256: return launch_gemm<256, false, false>(ta, tb, p, smem, st);
+      case 160: return launch_gemm<160, false, false>(ta, tb, p, smem, st);
+      case 128: return launch_gemm<128, false, false>(ta, tb, p, smem, st);
+      case 64:  return launch_gemm<64, false, false>(ta, tb, p, smem, st);
     }
   }
   return set_error("glg_gemm: internal: bad tile");

@@ -15,11 +15,12 @@ int check_launch(const char* what);
 // bf16 tiled tensor map with 128B swizzle and zero out-of-bounds fill (host-side cache keyed by all
 // arguments).  dims/box innermost first; strides in BYTES for dims 1..rank-1.  Returns 0 or records the error.
 int get_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box);
+// swizzle_bytes: 0 (none), 64 or 128; rank 1..5
 int get_tmap_bf16_sw(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box, int swizzle_bytes);
 int num_sms();
-bool pdl_enabled();     // GLG_PDL env (default off: measured neutral-to-negative for this launch mix)
+bool pdl_enabled();     // GLG_PDL env (default off)
 int pdl_mode();         // 0 off, 1 every launch, 2 only launches whose grid leaves SMs idle (fewer CTAs than SMs): their prologue
-                        // (launch latency, barrier init, TMEM allocation) overlaps the tail of the kernel before them
+                        // (launch latency, barrier init) overlaps the tail of the kernel before them
 
 // Launch with programmatic dependent launch (and optionally a thread-block cluster along x).
 template <typename... KArgs, typename... Args>

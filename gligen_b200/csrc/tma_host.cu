@@ -29,7 +29,7 @@ static PFN_encodeTiled get_encode_fn() {
 }
 
 struct TmapKey {
-  const void* ptr; uint64_t d[4]; uint64_t s[3]; uint32_t box[4]; int rank; int swizzle;
+  const void* ptr; uint64_t d[5]; uint64_t s[4]; uint32_t box[5]; int rank; int swizzle;
   bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
 };
 struct TmapKeyHash {
@@ -49,7 +49,7 @@ int get_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* d
   return get_tmap_bf16_sw(out, ptr, rank, dims, strides, box, 128);
 }
 
-// same with the swizzle width chosen by the caller (64: the epilogue's [32 x 32] staging chunks, inner box = 64 bytes)
+// same with the swizzle width chosen by the caller (0: none, 64 or 128 bytes); rank up to 5
 int get_tmap_bf16_sw(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides,
                      const uint32_t* box, int swizzle_bytes) {
   TmapKey key;
@@ -62,12 +62,14 @@ int get_tmap_bf16_sw(CUtensorMap* out, const void* ptr, int rank, const uint64_t
   if (it != g_tmaps.end()) { *out = it->second; return 0; }
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) return set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t gd[4]; cuuint64_t gs[3]; cuuint32_t bx[4]; cuuint32_t es[4] = {1, 1, 1, 1};
+  if (rank < 1 || rank > 5) return set_error("tensor map rank must be 1..5");
+  cuuint64_t gd[5]; cuuint64_t gs[4]; cuuint32_t bx[5]; cuuint32_t es[5] = {1, 1, 1, 1, 1};
   for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; }
   for (int i = 0; i < rank - 1; ++i) gs[i] = strides[i];
   CUtensorMap m;
   CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), gd, gs, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   swizzle_bytes == 0 ? CU_TENSOR_MAP_SWIZZLE_NONE : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char buf[256];
@@ -90,7 +92,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }

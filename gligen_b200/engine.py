@@ -2,7 +2,7 @@
 a flat list of kernel launches (a "plan") that is replayed - directly or as a CUDA graph - every step.
 
 Mirrors UNetModel.forward (reference ldm/modules/diffusionmodules/openaimodel.py:420-464) with these
-B200-first restructurings, all exact in real arithmetic:
+restructurings, all exact in real arithmetic:
   * channels-last bf16 activations; [B,C,H,W] <-> [B,(HW),C] rearranges of SpatialTransformer
     (attention.py:371,374) disappear;
   * skip connections are written by their producer straight into the channel slice of the concat buffer

@@ -8,13 +8,13 @@ inpainting front end `autoencoder.encode(image)`, gligen_inference.py:403-404).
     Upsample.forward          model.py:53-57     (nearest x2, then 3x3 conv)
 
 Same building blocks as the UNet engine: channels-last bf16 activations, GroupNorm(+SiLU) as the single-launch kernel,
-every 3x3 / 1x1 convolution as the tcgen05 implicit GEMM with bias / residual in its epilogue (tiles that are segments
+every 3x3 / 1x1 convolution as the wgmma implicit GEMM with bias / residual in its epilogue (tiles that are segments
 of one image row for the 256- and 512-wide levels), nearest upsample as one gather pass.  Restructurings, exact in real
 arithmetic:
   * z / scale_factor -> post_quant_conv (1x1) -> conv_in (3x3) is ONE 3x3 convolution over [z, 1]: the 1x1 weights and
     1 / scale_factor are folded into the 3x3 weights; post_quant_conv's bias travels through a constant ones channel so
     that the zero padding of conv_in still sees zeros outside the image;
-  * the mid attention has one head of dim 512 (O would not fit TMEM next to S), so it runs as three GEMMs with an fp32
+  * the mid attention has one head of dim 512 (O would not fit in registers next to S), so it runs as three GEMMs with an fp32
     score matrix and a row-softmax kernel between them:  S = Q K^T,  P = softmax(S * C^-1/2),  O = P V  with
     V^T = W_v hn^T produced directly in the [C, HW] layout the second GEMM wants; the bias of v is added after P.V
     (rows of P sum to 1).

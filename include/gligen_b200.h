@@ -39,7 +39,7 @@ int64_t glg_launch_count(void);
 void glg_reset_launch_count(void);
 
 /* ---- tensor-core GEMM / implicit-GEMM convolution -------------------------------------------
- * out[M,N] = epilogue( A[M,K] * W[N,K]^T )      tcgen05.mma (bf16 x bf16 -> fp32 in TMEM), TMA-fed.
+ * out[M,N] = epilogue( A[M,K] * W[N,K]^T )      wgmma (bf16 x bf16 -> fp32 in registers), TMA-fed.
  *
  * Replaces: nn.Linear (attention.py:110-115,161-165,42,61,239), nn.Conv2d 1x1 (attention.py:349,360;
  * openaimodel.py:194), nn.Conv2d 3x3 stride 1 (openaimodel.py:157,183,70; conv_mode=1), the
@@ -106,10 +106,9 @@ int glg_gemm(const GlgGemmArgs* args, void* stream);
  * attention over [visual ; grounding] tokens with only the first Lq query rows kept, :241).
  * q/k/v are bf16 with independent row strides (elements) and batch strides so that packed QKV / KV
  * GEMM outputs are consumed in place.  d_head in {8,16,...,160}, multiple of 8.
- * Kernel selection (csrc/attention_tc.cu, csrc/attention.cu): d_head <= 128 and Lk > 128 -> tcgen05/TMEM kernel (needs
- * 16-byte aligned q/k/v/out and strides that are multiples of 8 elements); Lk <= 128 (the 77-token text context) ->
- * K/V-resident mma.sync kernel; d_head > 128 -> streaming mma.sync kernel.  All three give the same result to bf16
- * round-off (tests/test_kernels_gpu.py::test_attention runs them against each other's reference).
+ * Kernel selection (csrc/attention.cu): Lk <= 128 (the 77-token text context) -> K/V-resident mma.sync kernel;
+ * longer key sets -> wgmma + TMA flash kernel.  All kernels give the same result to bf16 round-off
+ * (tests/test_kernels_gpu.py::test_attention runs each against the same reference).
  */
 typedef struct GlgAttnArgs {
   const void* q; const void* k; const void* v; void* out;   /* bf16 */

@@ -1,5 +1,5 @@
 """`AutoencoderKL` at the reference's import path (ldm/models/autoencoder.py:17-44), with `decode` and `encode` on this
-repo's sm_100a kernels (gligen_b200/vae.py).  What gligen_inference.py does with it: `instantiate_from_config(config['autoencoder'])
+repo's sm_90a kernels (gligen_b200/vae.py).  What gligen_inference.py does with it: `instantiate_from_config(config['autoencoder'])
 .to(device).eval()`, `load_state_dict(saved_ckpt["autoencoder"])` (:76-84), `autoencoder.decode(samples_fake)` (:441) and, for
 inpainting only, `autoencoder.encode(...)` (:403).
 
@@ -30,7 +30,7 @@ class _CudaDecodeMixin:
     def _vae_engine(self):
         dev = self.post_quant_conv_weight_device()
         if dev.type != "cuda":
-            raise RuntimeError("gligen_b200 AutoencoderKL.decode runs only on a CUDA device (sm_100a kernels); call .to('cuda') first")
+            raise RuntimeError("gligen_b200 AutoencoderKL.decode runs only on a CUDA device (sm_90a kernels); call .to('cuda') first")
         if getattr(self, "_glg_engine", None) is None or self._glg_engine.dev != dev:
             from gligen_b200.ops import CudaOps
             from gligen_b200.vae import VAEDecoderEngine
@@ -56,7 +56,7 @@ class _CudaDecodeMixin:
     def _vae_enc_engine(self):
         dev = self.post_quant_conv_weight_device()
         if dev.type != "cuda":
-            raise RuntimeError("gligen_b200 AutoencoderKL.encode runs only on a CUDA device (sm_100a kernels); call .to('cuda') first")
+            raise RuntimeError("gligen_b200 AutoencoderKL.encode runs only on a CUDA device (sm_90a kernels); call .to('cuda') first")
         if getattr(self, "_glg_enc", None) is None or self._glg_enc.dev != dev:
             from gligen_b200.ops import CudaOps
             from gligen_b200.vae import VAEEncoderEngine

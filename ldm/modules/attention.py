@@ -3,7 +3,7 @@
 In this engine these classes are parameter containers only: the arithmetic of
 reference ldm/modules/attention.py (SelfAttention :154-186, CrossAttention :102-149,
 GatedSelfAttentionDense :215-244, BasicTransformerBlock :303-338, SpatialTransformer :341-376) runs as
-fused sm_100a kernels driven by gligen_b200.engine; the containers exist so that
+fused sm_90a kernels driven by gligen_b200.engine; the containers exist so that
   * state_dict() keys equal the reference's (checkpoints load verbatim), and
   * `set_alpha_scale` (gligen_inference.py:24-28), which walks model.modules() and tests
     `type(module) == GatedSelfAttentionDense`, finds the fusers and sets `.scale` on them.

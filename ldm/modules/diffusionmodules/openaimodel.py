@@ -4,7 +4,7 @@ located by string through instantiate_from_config; reference openaimodel.py:237-
 Same constructor kwargs, same state_dict keys/shapes, same `forward(input: dict) -> eps` contract, same
 externally visible attributes (`image_size`, `in_channels`, `inpaint_mode`, `grounding_tokenizer_input`,
 `first_conv_type`, `restore_first_conv_from_SD`, fuser modules with `.scale`).  The arithmetic is NOT
-PyTorch: forward() hands raw device pointers to libgligen_b200.so (hand-written sm_100a kernels) through
+PyTorch: forward() hands raw device pointers to libgligen_b200.so (hand-written sm_90a kernels) through
 gligen_b200.engine.  There is no CPU / eager fallback: parameters must live on a CUDA device.
 """
 import os
@@ -165,7 +165,7 @@ class UNetModel(ParamNode):
         """The native engine bound to this module's parameters (built lazily on the parameters' device)."""
         dev = self.time_embed[0].weight.device
         if dev.type != "cuda":
-            raise RuntimeError("gligen_b200 UNetModel runs only on a CUDA device (sm_100a kernels); "
+            raise RuntimeError("gligen_b200 UNetModel runs only on a CUDA device (sm_90a kernels); "
                                "there is no CPU fallback - call .to('cuda') first")
         if self._engine is None:
             from gligen_b200.engine import Engine

@@ -1,5 +1,5 @@
 """`FrozenCLIPEmbedder` at the reference's import path (ldm/modules/encoders/modules.py:144-173; located by string through
-`instantiate_from_config(config['text_encoder'])`, gligen_inference.py:77), with the CLIP text transformer on this repo's sm_100a
+`instantiate_from_config(config['text_encoder'])`, gligen_inference.py:77), with the CLIP text transformer on this repo's sm_90a
 kernels (gligen_b200/clip_text.py).  Same surface: `FrozenCLIPEmbedder(version, device, max_length)`, `.to(device).eval()`,
 `load_state_dict(saved_ckpt["text_encoder"])` with the `transformer.text_model.*` keys of transformers' CLIPTextModel,
 `encode(text, return_pooler_output=False)` / `forward(...)` -> last_hidden_state [B, 77, 768] (, pooler_output).
@@ -70,7 +70,7 @@ class FrozenCLIPEmbedder(AbstractEncoder):
     def engine(self) -> ClipTextEngine:
         dev = self.transformer.text_model.final_layer_norm.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("gligen_b200 FrozenCLIPEmbedder runs only on a CUDA device (sm_100a kernels); call .to('cuda') first")
+            raise RuntimeError("gligen_b200 FrozenCLIPEmbedder runs only on a CUDA device (sm_90a kernels); call .to('cuda') first")
         if self._engine is None:
             from gligen_b200.ops import CudaOps
             self._engine = ClipTextEngine(self.cfg, CudaOps(dev))

@@ -5,7 +5,7 @@
 The reference (gligen/GLIGEN) is a pure-Python script tree without setup.py / pyproject.toml, so there is nothing
 to compile or pip-install; the equivalent of "building the reference into oracle/_ref" is an import-able archive of
 its modules, byte for byte as they lie under /root/reference (python imports straight from a .zip).  The archive is
-git-ignored (it never enters history) but travels to the GPU box with the gpurun snapshot, where /root/reference does
+git-ignored (it never enters history); copied with the working tree to a GPU machine, where /root/reference does
 not exist.  Users (all of them checkers, never the product path):
 
   * bench.py --impl reference : times the reference's own PLMSSampler + UNetModel on the host cores;

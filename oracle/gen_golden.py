@@ -1,5 +1,5 @@
 """Pin the oracle against the REAL reference and write tests/golden/*.pt.   (run in the authoring
-container only; /root/reference does not exist on the GPU box)
+container only; /root/reference does not exist on the GPU machine)
 
     python oracle/gen_golden.py [--full] [--tiny]
 
@@ -346,6 +346,19 @@ def run_vae_encode(name, B, seed=5, store_half=False):
                os.path.join(GOLD, f"{name}_enc_B{B}.pt"))
 
 
+def convert_ckpt_add_channels():
+    """the reference's convert_ckpt.add_additional_channels on the seeded 320-channel first conv of
+    tests/test_checkpoint_cpu.py::test_inpaint_channel_surgery_matches_reference"""
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("_ref_convert_ckpt", os.path.join(REF, "convert_ckpt.py"))
+    ref = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(ref)
+    g = torch.Generator().manual_seed(0)
+    sd = {"input_blocks.0.0.weight": torch.randn(320, 4, 3, 3, generator=g), "other": torch.ones(2)}
+    ref.add_additional_channels(sd, 5)
+    torch.save({k: v.clone() for k, v in sd.items()}, os.path.join(GOLD, "convert_ckpt_add_channels.pt"))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--full", action="store_true")
@@ -381,13 +394,14 @@ if __name__ == "__main__":
         sys.exit(0)
     if args.tiny or not args.full:
         scalar_anchors()
+        convert_ckpt_add_channels()
         run_config("tiny", B=2, max_objs=6, plms_S=4, alpha_type=[0.5, 0, 0.5], ddim_S=2)
         run_config("tiny_text_image", B=2, max_objs=5, plms_S=4, alpha_type=[1, 0, 0], ddim_S=2)
         run_config("tiny_keypoint", B=2, max_objs=34, plms_S=4, alpha_type=[1, 0, 0], ddim_S=2)
         run_config("tiny_inpaint", B=2, max_objs=6, plms_S=4, alpha_type=[0.5, 0, 0.5], ddim_S=2)
     if args.full:
         # the SD first conv (real SD-1.4 weights bundled with the reference) is needed by the
-        # restore_first_conv_from_SD step on the GPU box: keep a copy as a data fixture.
+        # restore_first_conv_from_SD step on the GPU machine: keep a copy as a data fixture.
         w = torch.load(os.path.join(REF, "SD_input_conv_weight_bias.pth"))
         torch.save({"weight": w["weight"].clone(), "bias": w["bias"].clone()}, os.path.join(GOLD, "SD_input_conv_weight_bias.pth"))
         # BASELINE config 1: 1x4x64x64, 2 DDIM steps, 2 box+text tokens; plus PLMS S=4 with the

@@ -1,7 +1,7 @@
 """Drive the UNMODIFIED reference (gligen/GLIGEN) on the hot path.  TEST / BASELINE INFRASTRUCTURE ONLY.
 
 The reference modules come either from /root/reference (authoring container) or from the archive that
-oracle/build_ref.py writes (oracle/_ref/gligen_reference.zip, travels to the GPU box).  Nothing here is imported by the
+oracle/build_ref.py writes (oracle/_ref/gligen_reference.zip, copied with the working tree to a GPU machine).  Nothing here is imported by the
 product package; users are oracle/gen_golden.py, oracle/ref_run.py (CLI used by the GPU parity tests through a
 subprocess) and bench.py's `--impl reference` / `cpu_baseline` legs.
 
@@ -41,7 +41,7 @@ def _pin_namespace(name: str, path: str) -> None:
 
 def mount(prefer: str = "auto") -> str:
     """Make `ldm.*`, `grounding_input.*`, `inpaint_mask_func` resolve to REFERENCE code in this process.
-    prefer: "dir" (/root/reference), "zip" (oracle/_ref archive) or "auto" (dir when present).
+    prefer: "dir" (/root/reference), "zip" (oracle/_ref archive) or "auto" (the archive when present, else the dir).
     Returns the directory that holds SD_input_conv_weight_bias.pth (the reference reads it CWD-relative)."""
     global _mounted
     if _mounted:
@@ -49,7 +49,7 @@ def mount(prefer: str = "auto") -> str:
     if REPO not in sys.path:
         sys.path.insert(0, REPO)
     from oracle import build_ref
-    use_dir = os.path.isdir(REF_DIR) and prefer in ("auto", "dir")
+    use_dir = os.path.isdir(REF_DIR) and (prefer == "dir" or (prefer == "auto" and not build_ref.available()))
     if not use_dir and not build_ref.available():
         raise RuntimeError("reference unavailable: neither /root/reference nor oracle/_ref/gligen_reference.zip exists")
     for name in ("ldm", "grounding_input", "inpaint_mask_func"):

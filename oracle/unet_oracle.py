@@ -8,7 +8,7 @@ bench.py's cpu_baseline / `--impl reference` legs may import it.  The product pa
 Parity pinning: the reference has no tests or golden vectors of its own (SURVEY 4, 8c), so this
 restatement is pinned by EXECUTING the reference: oracle/gen_golden.py imports /root/reference,
 loads the same seeded weights into the reference `UNetModel`, asserts agreement with this file to
-fp32 round-off and writes tests/golden/*.pt, which travel to the GPU box.
+fp32 round-off and writes tests/golden/*.pt, which travel to the GPU machine.
 
 Every function cites the reference file:line it follows.
 """

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Once-per-image front / back end rows on one B200 (CUDA events, after warm-up): CLIP text encoder, ConvNeXt grounding tokenizer +
+"""Once-per-image front / back end rows on one GPU (CUDA events, after warm-up): CLIP text encoder, ConvNeXt grounding tokenizer +
 grounding downsampler (the static part of a spatial model's plan), VAE decode.  Prints one JSON line per item.
     python scripts/bench_frontend.py [B]"""
 import json, os, sys

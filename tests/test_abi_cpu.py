@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/gligen_b200.h declares
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/gligen_b200.h declares
 (no compute calls - there is no GPU here); the drop-in surface and host logic behave like the reference's."""
 import ctypes
 import os
@@ -26,15 +26,15 @@ def test_library_exports_every_declared_symbol():
     assert L.glg_launch_count() == 0
 
 
-def test_kernels_are_blackwell_native():
-    """SASS evidence: tcgen05.mma -> UTCHMMA, TMA -> UTMALDG, tcgen05.ld -> LDTM (B200_PROFILING.md)."""
+def test_kernels_are_hopper_native():
+    """SASS evidence: wgmma -> HGMMA, TMA loads -> UTMALDG (incl. the multicast of the paired GEMM), mma.sync -> HMMA."""
     import shutil
     import subprocess
     from gligen_b200 import build
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run(["cuobjdump", "-sass", build.build()], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
+    for mnemonic in ("HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "HMMA"):
         assert mnemonic in sass, mnemonic
 
 

@@ -1,6 +1,6 @@
 """bench.py contract pieces that run without a GPU: the reference arm (the real reference PLMSSampler + UNetModel from
-oracle/_ref or /root/reference on the host cores; the oracle port only when neither exists) prints one JSON line with the
-keys the driver reads; the product arm refuses to run without CUDA (no CPU fallback)."""
+the archive oracle/_ref that build() makes where the original project is available, on the host cores; the oracle port
+when it is absent) prints one JSON line with the keys the benchmark consumers read; the product arm refuses to run without CUDA (no CPU fallback)."""
 import json
 import os
 import subprocess
@@ -20,7 +20,8 @@ def test_reference_arm_line():
     assert line["value"] > 0 and line["e2e"]["value"] == line["value"]
     assert line["e2e"]["h2d_bytes_per_step"] == 0 and line["e2e"]["d2h_bytes_per_step"] == 0
     cb = line["cpu_baseline"]
-    have_ref = os.path.isdir("/root/reference") or os.path.exists(os.path.join(ROOT, "oracle", "_ref", "gligen_reference.zip"))
+    from oracle import build_ref, ref_harness
+    have_ref = build_ref.available() or os.path.isdir(ref_harness.REF_DIR)          # the rule ref_harness.mount("auto") uses
     assert cb["kind"] == ("reference" if have_ref else "port") and cb["cores"] >= 1 and cb["value"] == line["value"] and cb["sample"]
     if have_ref:
         assert "PLMSSampler.sample" in cb["sample"] and line["config"]["reference_batch"] >= 1

@@ -1,5 +1,5 @@
 """GPU: the CLIP text encoder (SURVEY 8f-3) through the C ABI against the library fixture (tests/golden/clip_text_*.pt), and the
-kernels it adds: causal mask of the short-key tcgen05 attention, token-embedding gather, fp32-output LayerNorm.
+kernels it adds: causal mask of the short-key attention kernel, token-embedding gather, fp32-output LayerNorm.
 Tolerance: 12 bf16 pre-LN blocks -> rel-L2 <= 1.5e-2, max-abs <= 6 % of max|z| on last_hidden_state and pooler_output (the UNet
 reads the context in bf16 anyway: `context.cast`)."""
 import os

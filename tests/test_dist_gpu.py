@@ -3,7 +3,7 @@ packed bf16 arena; the global batch sharded contiguously; NO collective on the p
 the latents of the 1-GPU run of the same global batch - within a stated tolerance, because the per-rank batch changes
 M and with it the GEMM tile / split-K choices (same bf16 math, different fp32 summation order).
 
-Needs 2 GPUs (`gpurun --gpus 2`); skipped on a single-GPU box."""
+Needs 2 GPUs; skipped on a single-GPU machine."""
 import os
 import sys
 

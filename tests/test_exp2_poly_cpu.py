@@ -1,4 +1,4 @@
-"""CPU: the FMA-pipe exp2 of the level-0 attention kernels (csrc/attention_tc3.cu ex2_poly3: Cody-Waite split by the 1.5 * 2^23 magic
+"""CPU: the FMA-pipe exp2 of the long-key attention kernels (csrc/common.cuh ex2_poly3: Cody-Waite split by the 1.5 * 2^23 magic
 constant + Taylor cubic on [-0.5, 0.5] + exponent insertion), restated in numpy fp32 exactly as the kernel computes it: relative error
 against exp2 over the whole range the softmax feeds it - 1.2e-4 on average, 7.9e-4 at worst (|f| = 0.5) - below the bf16 rounding of P
 (half an ulp = 2^-9 = 2e-3), and exact zero-ish results for masked / underflowing scores."""

@@ -8,8 +8,8 @@ Golden: tests/golden/sd14_box_text_B1_G30_plms50.pt - the UNMODIFIED reference r
 Denominator (SURVEY 8d "Parity gate"): the reference's OWN reduced-precision gap, measured in the same run on the same GPU:
 the reference under torch.autocast(bf16) (and fp16, fp32 eager for information) against the same fp32 golden, via
 oracle/ref_run.py on the archived reference (oracle/_ref).  Stated tolerance: max-abs and rel-L2 of the engine's final
-latent <= 2x the reference's bf16-autocast gap.  When the archive is not on the box the committed measurement
-(tests/golden/final_latent_gaps.json, written by this test on a box that had it) supplies the denominator."""
+latent <= 2x the reference's bf16-autocast gap.  When the archive is absent the committed measurement
+(tests/golden/final_latent_gaps.json, printed by this test where the archive was present) supplies the denominator."""
 import json
 import os
 import subprocess
@@ -79,11 +79,7 @@ def test_final_latent_plms50(atype, tmp_path):
     if refs is not None:
         rec.update({"reference_bf16_autocast": gap(refs["bf16"], ref), "reference_fp16_autocast": gap(refs["fp16"], ref),
                     "reference_fp32_gpu_eager": gap(refs["none"], ref), "denominator": "measured in this run (oracle/_ref on this GPU)"})
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        path = os.path.join(ROOT, "gpurun_out", "final_latent_gaps.json")
-        allrec = json.load(open(path)) if os.path.exists(path) else {}
-        allrec[key] = rec
-        json.dump(allrec, open(path, "w"), indent=1)
+        print(f"\nGAPS {json.dumps({key: rec})}")      # the record tests/golden/final_latent_gaps.json keeps per key
         den = rec["reference_bf16_autocast"]
     else:
         assert os.path.exists(GAPS_FILE), "neither oracle/_ref nor the committed denominator (tests/golden/final_latent_gaps.json) is present"

@@ -49,7 +49,7 @@ GEMM_CASES = [
 @pytest.mark.parametrize("force_bn", [0, 64, 128, 160, 256])
 @pytest.mark.parametrize("cta2", [0, 1, 2])
 def test_gemm(ops, ref, M, N, K, fl, force_bn, cta2):
-    """cta2: 0 = tile heuristic, 1 = single-CTA kernel (cta_group::1), 2 = paired kernel (cluster of 2, cta_group::2)."""
+    """cta2: 0 = tile heuristic, 1 = single-CTA kernel, 2 = paired kernel (cluster of 2, B tile multicast to both CTAs)."""
     if force_bn and (N % force_bn or fl.get("geglu")):
         pytest.skip("BN does not divide N")
     if force_bn and M > 5000:
@@ -295,21 +295,21 @@ ATTN_CASES = [
 ]
 
 
+# path -> (glg_debug_attn_mode, FMA-pipe exp2 share of 8).  The path names are those of the kernels of the
+# project's Blackwell build; each selects one H100 configuration: 0 = auto dispatch, 1 = streamed mma.sync kernel,
+# 2 = wgmma / TMA kernel, 3 = short-key mma.sync kernel.
+ATTN_PATHS = {"auto": (0, 0), "mma_sync": (1, 0), "tcgen05": (2, 0), "tcgen05_sum": (2, 1), "short_tc": (3, 0), "tc2": (2, 2), "tc3": (1, 2)}
+
+
 @pytest.mark.parametrize("B,heads,d,Lq,Lk,mode", ATTN_CASES)
 @pytest.mark.parametrize("path", ["auto", "mma_sync", "tcgen05", "tcgen05_sum", "short_tc", "tc2", "tc3"])
 def test_attention(ops, ref, B, heads, d, Lq, Lk, mode, path):
-    """auto: streamed tcgen05 flash kernel (> 128 keys, every d_head <= 160), short-key tcgen05 kernel (<= 128 keys: the
-    text context).  Row sums come from a ones column of V when d_head % 16 != 0 (streamed kernel).
-    The other paths force the legacy mma.sync kernel / the streamed tcgen05 kernel (also for short key sets) / the
-    streamed kernel with the softmax-side row sum."""
-    if path in ("tc2", "tc3") and (d % 16 == 0 or d > 64):
-        pytest.skip("multi-warpgroup kernels: d_head < 64 with a spare column for the row sums")
-    if path == "short_tc" and (Lk > 128 or d > 128 and Lk > 80):
-        pytest.skip("short-key kernel: all keys in one tile")
-    if path == "short_tc" and Lk <= 128:
-        pytest.skip("same kernel as auto")
-    if path == "tcgen05_sum" and d % 16 == 0:
-        pytest.skip("same kernel as tcgen05 / auto")
+    """auto: the short-key mma.sync kernel (K/V resident, <= 128 keys: the text context) or the wgmma / TMA flash kernel
+    (longer key sets).  The other paths force one kernel for every case it accepts (ATTN_PATHS): the streamed mma.sync
+    kernel, the wgmma kernel (also for short key sets), the short-key kernel (Lk <= 128 only); tcgen05_sum / tc2 / tc3 run
+    the wgmma or streamed kernel with 1 or 2 of every 8 score pairs exponentiated on the FMA pipe."""
+    if path == "short_tc" and Lk > 128:
+        pytest.skip("short-key kernel: all keys in at most two resident tiles")
     C = heads * d
     if mode == "qkv":
         qkv = rnd(B, Lk, 3 * C)
@@ -325,55 +325,8 @@ def test_attention(ops, ref, B, heads, d, Lq, Lk, mode, path):
         q, k, v = rnd(B, Lq, C), rnd(B, Lk, C, seed=1), rnd(B, Lk, C, seed=2)
     out = torch.zeros(B, Lq, C, device="cuda:0", dtype=torch.bfloat16)
     out_r = torch.zeros_like(out)
-    ops.lib.glg_debug_attn_mode({"auto": 0, "mma_sync": 1, "tcgen05": 2, "tcgen05_sum": 2, "short_tc": 3, "tc2": 4, "tc3": 5}[path])
-    ops.lib.glg_debug_attn_tc_variant(3 if path == "tcgen05_sum" else 0)
-    try:
-        ops.attention(q, k, v, out, heads, d)
-        torch.cuda.synchronize()
-    finally:
-        ops.lib.glg_debug_attn_mode(0)
-        ops.lib.glg_debug_attn_tc_variant(0)
-    ref.attention(q, k, v, out_r, heads, d)
-    assert_close(out, out_r, rel=1e-2, max_rel=5e-2, what=f"attention d={d} {Lq}x{Lk} {mode}")
-
-
-@pytest.mark.parametrize("var", [0, 1, 3, 5, 7, 10, 18, 26])
-def test_attention_tc3_variants(ops, ref, var):
-    """three-tile kernel, FMA-pipe share 2/8, with the measured variants of the per-tile chain (lane-0 mbarrier waits, exponentials
-    before the wait for the previous P.V, lane-0 waits in the issuer warps): same results as the torch statement."""
-    B, heads, d, Lq, Lk = 2, 8, 40, 1024, 1054
-    C = heads * d
-    qkv = rnd(B, Lk, 3 * C) * 2.0
-    q, k, v = qkv[:, :Lq, :C], qkv[:, :, C:2 * C], qkv[:, :, 2 * C:]
-    out = torch.zeros(B, Lq, C, device="cuda:0", dtype=torch.bfloat16)
-    out_r = torch.zeros_like(out)
-    ops.lib.glg_debug_attn_mode(5)
-    ops.lib.glg_debug_attn_poly_share(2)
-    ops.lib.glg_debug_attn_tc3_variant(var)
-    try:
-        ops.attention(q, k, v, out, heads, d)
-        torch.cuda.synchronize()
-    finally:
-        ops.lib.glg_debug_attn_mode(0)
-        ops.lib.glg_debug_attn_poly_share(0)
-        ops.lib.glg_debug_attn_tc3_variant(2)          # the default
-    ref.attention(q, k, v, out_r, heads, d)
-    assert_close(out, out_r, rel=1e-2, max_rel=5e-2, what=f"attention tc3 variant {var}")
-
-
-@pytest.mark.parametrize("mode", [4, 5])
-@pytest.mark.parametrize("poly", [1, 2, 3])
-def test_attention_fma_pipe_exp2(ops, ref, poly, mode):
-    """multi-warpgroup kernels with `poly` of every 8 score pairs exponentiated on the FMA pipe (Cody-Waite + Taylor cubic, rel error 1.2e-4 mean / 7.9e-4 max)."""
-    if mode == 5 and poly == 3:
-        pytest.skip("single-read kernel: shares 0..2")
-    B, heads, d, Lq, Lk = 2, 8, 40, 1024, 1054
-    C = heads * d
-    qkv = rnd(B, Lk, 3 * C) * 2.0                   # wider score range than the default cases
-    q, k, v = qkv[:, :Lq, :C], qkv[:, :, C:2 * C], qkv[:, :, 2 * C:]
-    out = torch.zeros(B, Lq, C, device="cuda:0", dtype=torch.bfloat16)
-    out_r = torch.zeros_like(out)
-    ops.lib.glg_debug_attn_mode(mode)
+    kernel, poly = ATTN_PATHS[path]
+    ops.lib.glg_debug_attn_mode(kernel)
     ops.lib.glg_debug_attn_poly_share(poly)
     try:
         ops.attention(q, k, v, out, heads, d)
@@ -382,7 +335,31 @@ def test_attention_fma_pipe_exp2(ops, ref, poly, mode):
         ops.lib.glg_debug_attn_mode(0)
         ops.lib.glg_debug_attn_poly_share(0)
     ref.attention(q, k, v, out_r, heads, d)
-    assert_close(out, out_r, rel=1e-2, max_rel=5e-2, what=f"attention tc2 poly={poly}")
+    assert_close(out, out_r, rel=1e-2, max_rel=5e-2, what=f"attention d={d} {Lq}x{Lk} {mode} {path}")
+
+
+@pytest.mark.parametrize("mode", [4, 5])
+@pytest.mark.parametrize("poly", [1, 2, 3])
+def test_attention_fma_pipe_exp2(ops, ref, poly, mode):
+    """long-key kernels with `poly` of every 8 score pairs exponentiated on the FMA pipe (Cody-Waite + Taylor cubic, rel error
+    1.2e-4 mean / 7.9e-4 max), on a wider score range than the default cases.  mode 4: the wgmma kernel, 5: the streamed
+    mma.sync kernel."""
+    B, heads, d, Lq, Lk = 2, 8, 40, 1024, 1054
+    C = heads * d
+    qkv = rnd(B, Lk, 3 * C) * 2.0
+    q, k, v = qkv[:, :Lq, :C], qkv[:, :, C:2 * C], qkv[:, :, 2 * C:]
+    out = torch.zeros(B, Lq, C, device="cuda:0", dtype=torch.bfloat16)
+    out_r = torch.zeros_like(out)
+    ops.lib.glg_debug_attn_mode({4: 2, 5: 1}[mode])
+    ops.lib.glg_debug_attn_poly_share(poly)
+    try:
+        ops.attention(q, k, v, out, heads, d)
+        torch.cuda.synchronize()
+    finally:
+        ops.lib.glg_debug_attn_mode(0)
+        ops.lib.glg_debug_attn_poly_share(0)
+    ref.attention(q, k, v, out_r, heads, d)
+    assert_close(out, out_r, rel=1e-2, max_rel=5e-2, what=f"attention poly={poly} mode={mode}")
 
 
 @pytest.mark.parametrize("B,HW,C,ld,eps,silu", [(2, 4096, 320, 320, 1e-5, True), (2, 1024, 960, 960, 1e-5, True),

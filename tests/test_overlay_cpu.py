@@ -1,4 +1,5 @@
-"""The documented drop-in recipe (INTEGRATION.md 1): this repo FIRST on sys.path, the reference checkout after it.
+"""The documented drop-in recipe (INTEGRATION.md 1): this repo FIRST on sys.path, the reference checkout after it (here:
+the original project's modules from the oracle/_ref archive, extracted).
 The hot-path modules must resolve to this repo, everything else of the reference must stay importable
 (ldm.models.autoencoder is what gligen_inference.load_ckpt instantiates next to the UNet, gligen_inference.py:70-86),
 and names the drop-in modules do not define must fall through to the reference (gligen_b200/_overlay.py)."""
@@ -11,7 +12,7 @@ import pytest
 
 from conftest import ROOT
 
-REF = "/root/reference"
+ARCHIVE = os.path.join(ROOT, "oracle", "_ref", "gligen_reference.zip")     # the original project's modules, written by build()
 
 SCRIPT = textwrap.dedent('''
     import sys
@@ -64,9 +65,13 @@ SCRIPT = textwrap.dedent('''
 ''')
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="needs the reference checkout (authoring container)")
+@pytest.mark.skipif(not os.path.exists(ARCHIVE), reason="needs oracle/_ref (build() makes it where the original project is available)")
 def test_repo_overlays_reference_checkout(tmp_path):
-    r = subprocess.run([sys.executable, "-c", SCRIPT % dict(repo=ROOT, ref=REF)], cwd=str(tmp_path), capture_output=True, text=True,
+    import zipfile
+    ref = str(tmp_path / "reference")                 # a checkout of the original project: its modules, byte for byte
+    with zipfile.ZipFile(ARCHIVE) as z:
+        z.extractall(ref)
+    r = subprocess.run([sys.executable, "-c", SCRIPT % dict(repo=ROOT, ref=ref)], cwd=str(tmp_path), capture_output=True, text=True,
                        env={k: v for k, v in os.environ.items() if k != "PYTHONPATH"})
     assert r.returncode == 0 and "overlay ok" in r.stdout, r.stdout + r.stderr
 
