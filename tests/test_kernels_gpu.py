@@ -292,12 +292,19 @@ ATTN_CASES = [
     (2, 8, 40, 200, 64, "plain"),          # one key tile: the second softmax warpgroup of the two-warpgroup kernel sees none
     (1, 8, 40, 384, 129, "plain"),         # three key tiles (2 + 1), last one a single key
     (1, 4, 56, 130, 640, "plain"),
+    (1, 4, 104, 300, 555, "plain"),       # head-dim padding 112
+    (2, 4, 104, 200, 77, "kv"),
+    (2, 4, 136, 256, 286, "fuser"),       # head-dim padding 144
+    (1, 4, 136, 128, 100, "plain"),
 ]
 
 
 # path -> (glg_debug_attn_mode, FMA-pipe exp2 share of 8).  The path names are those of the kernels of the
-# project's Blackwell build; each selects one H100 configuration: 0 = auto dispatch, 1 = streamed mma.sync kernel,
-# 2 = wgmma / TMA kernel, 3 = short-key mma.sync kernel.
+# project's Blackwell build, kept so that the test ids stay stable; each selects one H100 configuration:
+#   tcgen05 = the wgmma / TMA kernel, tcgen05_sum = wgmma with 1 of 8 exponentials on the FMA pipe,
+#   tc2 = wgmma with 2 of 8 on the FMA pipe, tc3 = the streamed mma.sync kernel with 2 of 8 on the FMA pipe,
+#   short_tc = the short-key mma.sync kernel.  Modes: 0 = auto dispatch, 1 = streamed mma.sync kernel,
+#   2 = wgmma / TMA kernel, 3 = short-key mma.sync kernel.
 ATTN_PATHS = {"auto": (0, 0), "mma_sync": (1, 0), "tcgen05": (2, 0), "tcgen05_sum": (2, 1), "short_tc": (3, 0), "tc2": (2, 2), "tc3": (1, 2)}
 
 
