@@ -8,6 +8,8 @@
 //   dwconv7_ln    depthwise 7x7 + bias + LayerNorm(eps 1e-6) in one pass (convnext.py:40-44)
 //   resize_plane  bicubic (A = -0.75, align_corners = False) / nearest resampling of NCHW fp32 planes (F.interpolate)
 //   conv2d_small  direct k x k convolution with <= 16 output channels on NCHW fp32 (+ SiLU), nearest resize fused in
+// and the CLIP towers' front / back ends: embed_tokens (text), clip_vision_embed (CLS + patches + positions + pre-LayerNorm) and
+// clip_image_head (post-LayerNorm of the CLS row, visual projection, GLIGEN's reprojection) for the image tower.
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <math.h>
@@ -337,6 +339,128 @@ __global__ void embed_tokens_kernel(const int64_t* __restrict__ ids, const float
   }
 }
 
+// ---- image-tower input rows (transformers CLIPVisionEmbeddings + pre_layrnorm); one warp per output row -------------------
+// row n*(P+1) + 0 is LN(cls + pos[0]), row n*(P+1) + 1 + p is LN(patch[n*P + p] + pos[1 + p]); the add is fp32 and the statistics
+// are two-pass fp32 in registers (as layernorm_rows_kernel), bf16 out.
+__global__ void __launch_bounds__(256) clip_vision_embed_kernel(const float* __restrict__ patch, long long ldp, const float* __restrict__ cls,
+                                                                const float* __restrict__ pos, const float* __restrict__ gamma,
+                                                                const float* __restrict__ beta, bf16* __restrict__ x, long long ldx,
+                                                                int N, int P, int C, float eps) {
+  pdl_trigger();
+  pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= (long long)N * (P + 1)) return;
+  const int t = (int)(row % (P + 1));
+  const long long n = row / (P + 1);
+  const float* src = t == 0 ? cls : patch + (n * P + t - 1) * ldp;
+  const float* pr = pos + (long long)t * C;
+  const int c8n = C >> 3;
+  float v[LNR_MAX_CHUNKS][8];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
+    const int c8 = lane + 32 * i;
+    if (c8 < c8n) {
+      const float4 a0 = *reinterpret_cast<const float4*>(src + c8 * 8), a1 = *reinterpret_cast<const float4*>(src + c8 * 8 + 4);
+      const float4 p0 = __ldg(reinterpret_cast<const float4*>(pr + c8 * 8)), p1 = __ldg(reinterpret_cast<const float4*>(pr + c8 * 8 + 4));
+      v[i][0] = a0.x + p0.x; v[i][1] = a0.y + p0.y; v[i][2] = a0.z + p0.z; v[i][3] = a0.w + p0.w;
+      v[i][4] = a1.x + p1.x; v[i][5] = a1.y + p1.y; v[i][6] = a1.z + p1.z; v[i][7] = a1.w + p1.w;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += v[i][j];
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float mean = s / (float)C;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
+    if (lane + 32 * i < c8n) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; q = fmaf(d, d, q); }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+  const float rstd = rsqrtf(q / (float)C + eps);
+#pragma unroll
+  for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
+    const int c8 = lane + 32 * i;
+    if (c8 < c8n) {
+      float o[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] = fmaf((v[i][j] - mean) * rstd, __ldg(gamma + c8 * 8 + j), __ldg(beta + c8 * 8 + j));
+      uint4 u;
+      u.x = pack_bf16x2(o[0], o[1]); u.y = pack_bf16x2(o[2], o[3]); u.z = pack_bf16x2(o[4], o[5]); u.w = pack_bf16x2(o[6], o[7]);
+      *reinterpret_cast<uint4*>(x + row * ldx + c8 * 8) = u;
+    }
+  }
+}
+
+// ---- image-tower head, one CTA per image, fp32 on CUDA cores (transformers CLIPVisionTransformer pooling + visual_projection,
+// then GLIGEN's reprojection).  Every reduction has a fixed order for a fixed blockDim, so results are bit-reproducible.
+constexpr int HEAD_THREADS = 256;
+__device__ __forceinline__ float head_block_sum(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();                                  // red[] may still be read by the previous call
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+  for (int w = 0; w < HEAD_THREADS / 32; ++w) s += red[w];
+  return s;
+}
+
+__global__ void __launch_bounds__(HEAD_THREADS) clip_image_head_kernel(const bf16* __restrict__ x, long long x_batch,
+                                                                       const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                                       const float* __restrict__ wproj, const float* __restrict__ proj,
+                                                                       float target_norm, float* __restrict__ pooled, float* __restrict__ embeds,
+                                                                       float* __restrict__ feature, int C, int D, float eps) {
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ float head_smem[];
+  float* y = head_smem;                             // [C]  post_layernorm(CLS row)
+  float* e = head_smem + C;                         // [D]  image_embeds
+  __shared__ float red[HEAD_THREADS / 32];
+  const int n = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bf16* xr = x + (long long)n * x_batch;      // the CLS token is row 0 of image n
+  float s = 0.f;
+  for (int c = tid; c < C; c += HEAD_THREADS) { const float v = __bfloat162float(xr[c]); y[c] = v; s += v; }
+  const float mean = head_block_sum(s, red) / (float)C;
+  float q = 0.f;
+  for (int c = tid; c < C; c += HEAD_THREADS) { const float d = y[c] - mean; q = fmaf(d, d, q); }
+  const float rstd = rsqrtf(head_block_sum(q, red) / (float)C + eps);
+  for (int c = tid; c < C; c += HEAD_THREADS) {
+    const float v = fmaf((y[c] - mean) * rstd, gamma[c], beta[c]);
+    y[c] = v;
+    pooled[(long long)n * C + c] = v;
+  }
+  __syncthreads();
+  // image_embeds[d] = y . wproj[d, :]: one warp per output, lanes stride the row (coalesced), butterfly sum
+  for (int d = warp; d < D; d += HEAD_THREADS / 32) {
+    const float* wr = wproj + (long long)d * C;
+    float a = 0.f;
+    for (int c = lane; c < C; c += 32) a = fmaf(y[c], __ldg(wr + c), a);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) { e[d] = a; embeds[(long long)n * D + d] = a; }
+  }
+  if (proj == nullptr) return;
+  __syncthreads();
+  // f[j] = sum_d e[d] proj[d, j]: one thread per output column (coalesced rows of proj), sequential over d
+  float* f = feature + (long long)n * D;
+  float sq = 0.f;
+  for (int j = tid; j < D; j += HEAD_THREADS) {
+    float a = 0.f;
+    for (int d = 0; d < D; ++d) a = fmaf(e[d], __ldg(proj + (long long)d * D + j), a);
+    f[j] = a;
+    sq = fmaf(a, a, sq);
+  }
+  const float scale = target_norm / sqrtf(head_block_sum(sq, red));
+  for (int j = tid; j < D; j += HEAD_THREADS) f[j] *= scale;   // each thread rescales the columns it wrote
+}
+
 }  // namespace glg
 
 using namespace glg;
@@ -404,6 +528,32 @@ extern "C" int glg_embed_tokens(const int64_t* ids, const float* table, int64_t 
   launch_k(embed_tokens_kernel, dim3(fe_blocks(total, 256)), dim3(256), 0, ST, 1, ids, table, (long long)vocab, pos, (bf16*)out, (long long)ldo, B, L, C);
   count_launch();
   return check_launch("embed_tokens launch");
+}
+
+extern "C" int glg_clip_vision_embed(const float* patch, int64_t ldp, const float* cls, const float* pos, const float* gamma, const float* beta,
+                                     void* x, int64_t ldx, int32_t N, int32_t P, int32_t C, float eps, void* stream) {
+  if (C <= 0 || C % 8 || C > 256 * LNR_MAX_CHUNKS) return set_error("glg_clip_vision_embed: C must be a multiple of 8, <= 1024");
+  if (N < 0 || P < 0) return set_error("glg_clip_vision_embed: negative N or P");
+  if (ldp % 4 || ldx % 8 || (((uintptr_t)patch | (uintptr_t)cls | (uintptr_t)pos | (uintptr_t)x) & 15))
+    return set_error("glg_clip_vision_embed: ldp % 4, ldx % 8, 16-byte aligned pointers");
+  const long long rows = (long long)N * (P + 1);
+  if (rows == 0) return 0;
+  launch_k(clip_vision_embed_kernel, dim3((unsigned)((rows + 7) / 8)), dim3(256), 0, ST, 1, patch, (long long)ldp, cls, pos, gamma, beta,
+           (bf16*)x, (long long)ldx, N, P, C, eps);
+  count_launch();
+  return check_launch("clip_vision_embed launch");
+}
+
+extern "C" int glg_clip_image_head(const void* x, int64_t x_batch, const float* gamma, const float* beta, const float* w_proj, const float* proj,
+                                   float target_norm, float* pooled, float* embeds, float* feature, int32_t N, int32_t C, int32_t D, float eps,
+                                   void* stream) {
+  if (C <= 0 || D <= 0 || C + D > 12288) return set_error("glg_clip_image_head: need C, D > 0 and C + D <= 12288 (48 KiB of shared memory)");
+  if ((proj == nullptr) != (feature == nullptr)) return set_error("glg_clip_image_head: proj and feature go together");
+  if (N <= 0) return 0;
+  launch_k(clip_image_head_kernel, dim3((unsigned)N), dim3(HEAD_THREADS), (size_t)(C + D) * sizeof(float), ST, 1, (const bf16*)x, (long long)x_batch,
+           gamma, beta, w_proj, proj, target_norm, pooled, embeds, feature, C, D, eps);
+  count_launch();
+  return check_launch("clip_image_head launch");
 }
 
 extern "C" int glg_dwconv7_ln(const void* x, int64_t ldx, void* y, int64_t ldy, const float* w, const float* bias, const float* gamma,

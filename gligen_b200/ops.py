@@ -262,6 +262,31 @@ class CudaOps:
         L.check(self._c.glg_embed_tokens(ids.data_ptr(), table.data_ptr(), table.shape[0], pos.data_ptr(), op, ldo, B, Lt, Cc, self._stream()), "glg_embed_tokens")
         self._note("embed_tokens")
 
+    def clip_vision_embed(self, patch, cls, pos, gamma, beta, x, P: int, eps: float):
+        """x bf16 rows [N*(P+1), C]: row n*(P+1) = LN(cls + pos[0]), row n*(P+1)+1+p = LN(patch[n*P+p] + pos[1+p]); patch fp32 [N*P, C]."""
+        pp, rows, Cc, ldp = _rows_view(patch)
+        xp, xrows, _, ldx = _rows_view(x)
+        assert patch.dtype == torch.float32 and rows % P == 0 and xrows == rows // P * (P + 1)
+        assert cls.is_contiguous() and pos.is_contiguous() and pos.shape == (P + 1, Cc)
+        L.check(self._c.glg_clip_vision_embed(pp, ldp, cls.data_ptr(), pos.data_ptr(), gamma.data_ptr(), beta.data_ptr(), xp, ldx, rows // P, P, Cc,
+                                               eps, self._stream()), "glg_clip_vision_embed")
+        self._note("clip_vision_embed", 0.0, 2.0 * xrows * Cc * 5)
+
+    def clip_image_head(self, x, gamma, beta, w_proj, pooled, embeds, proj=None, feature=None, target_norm: float = 28.7, eps: float = 1e-5):
+        """x bf16 [N, T, C] (row 0 of each image is read): pooled fp32 [N, C] = LN(x[:, 0]), embeds fp32 [N, D] = pooled w_proj^T,
+        feature fp32 [N, D] = target_norm * f / |f| with f = embeds proj (when proj is given)."""
+        N, _, Cc = x.shape
+        D = w_proj.shape[0]
+        assert x.stride(-1) == 1 and w_proj.is_contiguous() and w_proj.shape == (D, Cc)
+        assert pooled.is_contiguous() and pooled.shape == (N, Cc) and embeds.is_contiguous() and embeds.shape == (N, D)
+        assert (proj is None) == (feature is None)
+        if proj is not None:
+            assert proj.is_contiguous() and proj.shape == (D, D) and feature.is_contiguous() and feature.shape == (N, D)
+        L.check(self._c.glg_clip_image_head(x.data_ptr(), x.stride(0), gamma.data_ptr(), beta.data_ptr(), w_proj.data_ptr(), _ptr(proj),
+                                             float(target_norm), pooled.data_ptr(), embeds.data_ptr(), _ptr(feature), N, Cc, D, eps, self._stream()),
+                "glg_clip_image_head")
+        self._note("clip_image_head", 2.0 * N * D * (Cc + (D if proj is not None else 0)), 4.0 * D * (Cc + D))
+
     def dwconv7_ln(self, x, y, w, bias, gamma, beta, B: int, H: int, W: int, C: int, eps: float):
         """depthwise 7x7 + bias + LayerNorm over the first C channels: x, y bf16 rows [B*H*W, Cpad]; w fp32 [49, C]."""
         xp, _, _, ldx = _rows_view(x)

@@ -5,7 +5,9 @@
     (gligen_inference.py:70-86, 346-349) with the yaml `params` as plain dicts (configs/*.yaml);
   * `set_alpha_scale` (gligen_inference.py:24-28) and `alpha_generator` (:31-66) - restated because the script itself
     needs `clip` / `omegaconf` to import (absent offline);
-  * `sampler_inputs(...)`: the `input` dict / mask / x0 of `run()` (:384-430) from synthetic embeddings.
+  * `sampler_inputs(...)`: the `input` dict / mask / x0 of `run()` (:384-430) from synthetic embeddings;
+  * `prepare_batch(meta, batch, max_objs, encoder)` (:146-187): the box + text + image grounding batch, CLIP features from
+    gligen_b200.clip_grounding.ClipGroundingEncoder.
 
 Shared by bench.py, __graft_entry__.smoke() and the GPU parity tests, so the benchmark never imports the test tree.
 """
@@ -117,3 +119,54 @@ def sampler_inputs(cfg: UNetConfig, model, tensors: Dict[str, torch.Tensor], bat
     input = dict(x=tensors["x"].clone(), timesteps=None, context=tensors["context"], grounding_input=grounding,
                  inpainting_extra_input=extra, grounding_extra_input=gextra)
     return input, mask, x0
+
+
+def prepare_batch(meta, batch: int = 1, max_objs: int = 30, encoder=None) -> Dict[str, torch.Tensor]:
+    """gligen_inference.py:146-187 with the features from `encoder` (a gligen_b200.clip_grounding.ClipGroundingEncoder): all
+    phrases in one text forward, all images in one image forward.  meta: "locations" (xyxy boxes), "phrases" and / or "images" (None entries allowed), optional "text_mask" /
+    "image_mask" (a number or a per-object list, complete_mask :131-142).  Returns boxes, masks, text_masks, image_masks,
+    text_embeddings, image_embeddings repeated over `batch`, on the encoder's device."""
+    if encoder is None:
+        raise ValueError("prepare_batch needs a ClipGroundingEncoder (its weights come from a CLIPModel state dict)")
+    phrases, images = meta.get("phrases"), meta.get("images")
+    images = [None] * len(phrases) if images is None else images
+    phrases = [None] * len(images) if phrases is None else phrases
+    locations = meta["locations"]
+    assert len(locations) <= max_objs
+    dev = encoder.device
+    boxes = torch.zeros(max_objs, 4)
+    masks = torch.zeros(max_objs)
+    text_masks = torch.zeros(max_objs)
+    image_masks = torch.zeros(max_objs)
+    text_embeddings = torch.zeros(max_objs, encoder.text_dim, device=dev)
+    image_embeddings = torch.zeros(max_objs, encoder.image_dim, device=dev)
+    n = min(len(locations), len(phrases), len(images))     # the reference zips locations with the features (:168)
+    t_idx = [i for i in range(n) if phrases[i] is not None]
+    i_idx = [i for i in range(n) if images[i] is not None]
+    if t_idx:
+        text_embeddings[t_idx] = encoder.text_features(encoder.phrase_ids([phrases[i] for i in t_idx]))
+        text_masks[t_idx] = 1
+    if i_idx:
+        image_embeddings[i_idx] = encoder.image_features(encoder.pixel_values([images[i] for i in i_idx]))
+        image_masks[i_idx] = 1
+    for idx, box in enumerate(locations[:n]):
+        boxes[idx] = torch.tensor(box)
+        masks[idx] = 1
+
+    def complete_mask(has_mask):
+        mask = torch.ones(1, max_objs)
+        if has_mask is None:
+            return mask
+        if isinstance(has_mask, (int, float)):
+            return mask * has_mask
+        for idx, value in enumerate(has_mask):
+            mask[0, idx] = value
+        return mask
+
+    out = {"boxes": boxes.unsqueeze(0).repeat(batch, 1, 1),
+           "masks": masks.unsqueeze(0).repeat(batch, 1),
+           "text_masks": text_masks.unsqueeze(0).repeat(batch, 1) * complete_mask(meta.get("text_mask")),
+           "image_masks": image_masks.unsqueeze(0).repeat(batch, 1) * complete_mask(meta.get("image_mask")),
+           "text_embeddings": text_embeddings.unsqueeze(0).repeat(batch, 1, 1),
+           "image_embeddings": image_embeddings.unsqueeze(0).repeat(batch, 1, 1)}
+    return {k: v.to(dev) for k, v in out.items()}

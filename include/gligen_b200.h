@@ -192,6 +192,22 @@ int glg_layernorm_rows_f32(const void* x, int64_t ldx, float* y, int64_t ldy, co
  * out[b, l, :] = bf16(table[ids[b, l], :] + pos[l, :]);  ids int64 [B, L], table fp32 [vocab, C], pos fp32 [L, C]. */
 int glg_embed_tokens(const int64_t* ids, const float* table, int64_t vocab, const float* pos, void* out, int64_t ldo, int32_t B, int32_t L,
                      int32_t C, void* stream);
+/* Image-tower input rows (gligen_inference.py:151-153,110 -> transformers CLIPVisionEmbeddings.forward + CLIPVisionTransformer
+ * pre_layrnorm): for image n of N with P patches, row n*(P+1) of x is LN(cls + pos[0]) and row n*(P+1)+1+p is
+ * LN(patch[n*P + p] + pos[1+p]).  patch fp32 [N*P, ldp] (the patch-embedding GEMM's fp32 output), cls fp32 [C], pos fp32 [P+1, C];
+ * the add is fp32, the statistics two-pass fp32, x bf16 rows of stride ldx.  One launch replaces cat + position add + LayerNorm. */
+int glg_clip_vision_embed(const float* patch, int64_t ldp, const float* cls, const float* pos, const float* gamma, const float* beta,
+                          void* x, int64_t ldx, int32_t N, int32_t P, int32_t C, float eps, void* stream);
+/* Image-tower head, fp32 on CUDA cores, one CTA per image (transformers CLIPVisionTransformer pooled_output = post_layernorm(CLS),
+ * CLIPVisionModelWithProjection visual_projection; gligen_inference.py:110 outputs.image_embeds, :114-116 the reprojection):
+ *   pooled[n]  = LN(x[n*x_batch + 0 : C])                              (bf16 CLS row in, two-pass fp32 statistics)
+ *   embeds[n]  = pooled[n] . w_proj^T                                  (w_proj fp32 [D, C], no bias)
+ *   feature[n] = f * target_norm / |f|_2,  f = embeds[n] . proj        (proj fp32 [D, D] as torch.load('projection_matrix'); optional:
+ *                                                                       proj and feature both NULL skips it)
+ * Reductions run in a fixed order: results are bit-reproducible.  (C + D) * 4 bytes of shared memory, <= 48 KiB. */
+int glg_clip_image_head(const void* x, int64_t x_batch, const float* gamma, const float* beta, const float* w_proj, const float* proj,
+                        float target_norm, float* pooled, float* embeds, float* feature, int32_t N, int32_t C, int32_t D, float eps,
+                        void* stream);
 /* ConvNeXt block front (convnext.py:40-43): depthwise 7x7 pad 3 + bias, then LayerNorm over channels, one pass.
  * x / y NHWC bf16; w fp32 packed [49][C] (tap-major); y columns [C, Cpad) are zeros. */
 int glg_dwconv7_ln(const void* x, int64_t ldx, void* y, int64_t ldy, const float* w, const float* bias, const float* gamma,

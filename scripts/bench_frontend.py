@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Once-per-image front / back end rows on one GPU (CUDA events, after warm-up): CLIP text encoder, ConvNeXt grounding tokenizer +
+"""Once-per-image front / back end rows on one GPU (CUDA events, after warm-up): CLIP text encoder, CLIP image tower with the
+GLIGEN reprojection (1 and 30 images, with the GPU name and power limit of the run), ConvNeXt grounding tokenizer +
 grounding downsampler (the static part of a spatial model's plan), VAE decode.  Prints one JSON line per item.
     python scripts/bench_frontend.py [B]"""
 import json, os, sys
@@ -7,6 +8,8 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gligen_b200 import synth
 from gligen_b200.clip_text import SD14_CLIP_TEXT, ClipTextEngine, synthetic_clip_state_dict, synthetic_token_ids
+from gligen_b200.clip_vision import SD14_CLIP_VISION, ClipVisionEngine, synthetic_clip_vision_state_dict, synthetic_pixel_values, \
+    synthetic_projection_matrix
 from gligen_b200.engine import Engine
 from gligen_b200.ops import CudaOps
 from gligen_b200.spec import NAMED_CONFIGS, SPATIAL_MAP_KEY, synthetic_state_dict
@@ -37,6 +40,38 @@ ms = timed(lambda: clip.forward(ids))
 flops = 2 * B * 77 * 12 * (2 * 4 * 768 * 768 + 2 * 2 * 768 * 3072 + 4 * 77 * 768)
 print(json.dumps({"item": "clip_text_encoder", "sequences": 2 * B, "ms": round(ms, 3), "tflops": round(flops / ms / 1e9, 1),
                   "launches_per_call": (ops.launch_count() - n0) // 13}), flush=True)
+
+
+def gpu_identity():
+    """GPU name and enforced power limit (W), read in this run (NVML, read-only)."""
+    out = {"gpu": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(torch.cuda.current_device())
+        out["power_limit_w"] = round(pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0)
+    except Exception:
+        pass
+    return out
+
+
+# CLIP ViT-L/14 image tower + GLIGEN reprojection (prepare_batch's image features): 1 image and max_objs = 30 images
+vcfg = SD14_CLIP_VISION
+vis = ClipVisionEngine(vcfg, ops)
+vis.load_state_dict(synthetic_clip_vision_state_dict(vcfg, 0))
+proj = synthetic_projection_matrix(vcfg.projection, 0).to(dev)
+C, T = vcfg.width, vcfg.tokens
+flops_img = (2 * vcfg.patches * vcfg.k_pad * C + vcfg.layers * T * (2 * 4 * C * C + 2 * 2 * C * vcfg.ffn) + vcfg.layers * 4 * T * T * C
+             + 2 * C * vcfg.projection + 2 * vcfg.projection ** 2)
+ident = gpu_identity()
+for N in (1, 30):
+    px = synthetic_pixel_values(N, 1).to(dev)
+    n0 = ops.launch_count()
+    ms = timed(lambda: vis.grounding_features(px, proj))
+    print(json.dumps({"item": "clip_image_tower", "images": N, "ms": round(ms, 3), "tflops": round(N * flops_img / ms / 1e9, 1),
+                      "gflop_per_image": round(flops_img / 1e9, 1), "launches_per_call": (ops.launch_count() - n0) // 13, **ident}), flush=True)
+del vis
+torch.cuda.empty_cache()
 
 # spatial front end: static part of the plan (ConvNeXt tokenizer + downsampler + the usual text K/V, grounding K/V projections)
 for name in ("sd14_hed", "sd14_sem"):
