@@ -8,9 +8,8 @@ reference tree): CLIPTextTransformer = token + position embeddings, 12 pre-Layer
 position of the highest token id (the EOT token).  Restated in oracle/clip_oracle.py and pinned against the installed
 transformers' CLIPTextModel.
 
-Here: one gather kernel for the embeddings, LayerNorm rows, fused-QKV glg_gemm, the short-key attention kernel with
-its causal mask, out-projection / fc2 GEMMs with the residual add in the epilogue, fc1 with the quick_gelu epilogue.
-bf16 activations and weights, fp32 accumulation / statistics, fp32 output.
+Here: one gather kernel for the embeddings, the blocks of clip_encoder.py with the short-key attention kernel's causal
+mask, the final LayerNorm with fp32 output.  bf16 activations and weights, fp32 accumulation / statistics, fp32 output.
 """
 from __future__ import annotations
 
@@ -20,7 +19,7 @@ from typing import Dict, Tuple
 
 import torch
 
-ACT_QUICK_GELU = 3
+from .clip_encoder import ClipEncoderEngine, layer_param_shapes, synthetic_state_dict
 
 
 @dataclass(frozen=True)
@@ -45,37 +44,15 @@ def clip_text_param_shapes(cfg: ClipTextConfig, prefix: str = "transformer.") ->
     t = f"{prefix}text_model"
     p[f"{t}.embeddings.token_embedding.weight"] = (cfg.vocab_size, cfg.width)
     p[f"{t}.embeddings.position_embedding.weight"] = (cfg.max_length, cfg.width)
-    for i in range(cfg.layers):
-        l = f"{t}.encoder.layers.{i}"
-        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
-            p[f"{l}.self_attn.{n}.weight"], p[f"{l}.self_attn.{n}.bias"] = (cfg.width, cfg.width), (cfg.width,)
-        p[f"{l}.layer_norm1.weight"], p[f"{l}.layer_norm1.bias"] = (cfg.width,), (cfg.width,)
-        p[f"{l}.mlp.fc1.weight"], p[f"{l}.mlp.fc1.bias"] = (cfg.ffn, cfg.width), (cfg.ffn,)
-        p[f"{l}.mlp.fc2.weight"], p[f"{l}.mlp.fc2.bias"] = (cfg.width, cfg.ffn), (cfg.width,)
-        p[f"{l}.layer_norm2.weight"], p[f"{l}.layer_norm2.bias"] = (cfg.width,), (cfg.width,)
+    p.update(layer_param_shapes(cfg, f"{t}."))
     p[f"{t}.final_layer_norm.weight"], p[f"{t}.final_layer_norm.bias"] = (cfg.width,), (cfg.width,)
     return p
 
 
 def synthetic_clip_state_dict(cfg: ClipTextConfig, seed: int = 0, prefix: str = "transformer.") -> Dict[str, torch.Tensor]:
-    """Seeded fp32 weights: projections ~ N(0, 1/fan_in), embeddings ~ N(0, 0.02) / N(0, 0.01) (CLIP's init), norm scales 1 + 0.1 N,
-    biases 0.05 N; a few embedding channels are scaled up like the massive channels trained CLIP towers show."""
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    sd: Dict[str, torch.Tensor] = OrderedDict()
-    for key, shape in clip_text_param_shapes(cfg, prefix).items():
-        if key.endswith("token_embedding.weight"):
-            t = torch.randn(shape, generator=g) * 0.02
-            t[:, :: max(1, cfg.width // 4)] *= 8.0
-        elif key.endswith("position_embedding.weight"):
-            t = torch.randn(shape, generator=g) * 0.01
-        elif key.endswith(".bias"):
-            t = torch.randn(shape, generator=g) * 0.05
-        elif len(shape) == 1:
-            t = 1.0 + 0.1 * torch.randn(shape, generator=g)
-        else:
-            t = torch.randn(shape, generator=g) * (shape[1] ** -0.5)
-        sd[key] = t
-    return sd
+    """Seeded fp32 weights, the scheme of clip_encoder.synthetic_state_dict (CLIP's init); the token embedding carries the
+    scaled-up massive channels."""
+    return synthetic_state_dict(clip_text_param_shapes(cfg, prefix), seed, massive="token_embedding.weight")
 
 
 def synthetic_token_ids(cfg: ClipTextConfig, B: int, seed: int = 0) -> torch.Tensor:
@@ -89,20 +66,7 @@ def synthetic_token_ids(cfg: ClipTextConfig, B: int, seed: int = 0) -> torch.Ten
     return ids
 
 
-class ClipTextEngine:
-    def __init__(self, cfg: ClipTextConfig, ops):
-        self.cfg, self.ops, self.dev = cfg, ops, ops.device
-        self.adt = ops.act_dtype
-        self.W: Dict[str, torch.Tensor] = {}
-        self._ws: Dict[int, Dict[str, torch.Tensor]] = {}
-        self.loaded = False
-
-    def _a(self, t):
-        return t.detach().to(device=self.dev, dtype=self.adt).contiguous()
-
-    def _f(self, t):
-        return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()
-
+class ClipTextEngine(ClipEncoderEngine):
     def load_state_dict(self, sd: Dict[str, torch.Tensor]) -> None:
         """Accepts the keys of FrozenCLIPEmbedder (`transformer.text_model.*`), of CLIPTextModel (`text_model.*`) or bare; the
         `position_ids` buffer older transformers versions save is ignored."""
@@ -112,15 +76,7 @@ class ClipTextEngine:
         W.clear()
         W["tok"], W["pos"] = self._f(sd[pre + "embeddings.token_embedding.weight"]), self._f(sd[pre + "embeddings.position_embedding.weight"])
         assert W["tok"].shape == (cfg.vocab_size, cfg.width) and W["pos"].shape[1] == cfg.width
-        for i in range(cfg.layers):
-            l = f"{pre}encoder.layers.{i}"
-            W[f"{i}.ln1.g"], W[f"{i}.ln1.b"] = self._f(sd[f"{l}.layer_norm1.weight"]), self._f(sd[f"{l}.layer_norm1.bias"])
-            W[f"{i}.ln2.g"], W[f"{i}.ln2.b"] = self._f(sd[f"{l}.layer_norm2.weight"]), self._f(sd[f"{l}.layer_norm2.bias"])
-            W[f"{i}.qkv.w"] = self._a(torch.cat([sd[f"{l}.self_attn.{n}_proj.weight"] for n in ("q", "k", "v")], dim=0))
-            W[f"{i}.qkv.b"] = self._f(torch.cat([sd[f"{l}.self_attn.{n}_proj.bias"] for n in ("q", "k", "v")], dim=0))
-            W[f"{i}.out.w"], W[f"{i}.out.b"] = self._a(sd[f"{l}.self_attn.out_proj.weight"]), self._f(sd[f"{l}.self_attn.out_proj.bias"])
-            W[f"{i}.fc1.w"], W[f"{i}.fc1.b"] = self._a(sd[f"{l}.mlp.fc1.weight"]), self._f(sd[f"{l}.mlp.fc1.bias"])
-            W[f"{i}.fc2.w"], W[f"{i}.fc2.b"] = self._a(sd[f"{l}.mlp.fc2.weight"]), self._f(sd[f"{l}.mlp.fc2.bias"])
+        self._load_layers(sd, pre)
         W["lnf.g"], W["lnf.b"] = self._f(sd[pre + "final_layer_norm.weight"]), self._f(sd[pre + "final_layer_norm.bias"])
         self.loaded = True
 
@@ -142,18 +98,10 @@ class ClipTextEngine:
         assert L <= c.max_length and L <= 128
         ws = self._workspace(B, L)
         ws["ids"].copy_(input_ids)
-        x, t, qkv, ao, h, z = ws["x"], ws["t"], ws["qkv"], ws["ao"], ws["h"], ws["z"]
-        C, d = c.width, c.width // c.heads
+        x, z = ws["x"], ws["z"]
         ops.embed_tokens(ws["ids"], W["tok"], W["pos"], x)
-        for i in range(c.layers):
-            ops.layernorm_rows(x, t, W[f"{i}.ln1.g"], W[f"{i}.ln1.b"], C, c.eps)
-            ops.gemm(t, W[f"{i}.qkv.w"], qkv.view(B * L, 3 * C), bias=W[f"{i}.qkv.b"])
-            ops.attention(qkv[:, :, :C], qkv[:, :, C: 2 * C], qkv[:, :, 2 * C:], ao, c.heads, d, causal=True)
-            ops.gemm(ao.view(B * L, C), W[f"{i}.out.w"], x, bias=W[f"{i}.out.b"], residual=x)
-            ops.layernorm_rows(x, t, W[f"{i}.ln2.g"], W[f"{i}.ln2.b"], C, c.eps)
-            ops.gemm(t, W[f"{i}.fc1.w"], h, bias=W[f"{i}.fc1.b"], act=ACT_QUICK_GELU)
-            ops.gemm(h, W[f"{i}.fc2.w"], x, bias=W[f"{i}.fc2.b"], residual=x)
-        ops.layernorm_rows_f32(x, z.view(B * L, C), W["lnf.g"], W["lnf.b"], c.eps)
+        self._run_layers(ws, causal=True)
+        ops.layernorm_rows_f32(x, z.view(B * L, c.width), W["lnf.g"], W["lnf.b"], c.eps)
         out = z.clone()
         # pooler_output: the hidden state at the (first) position of the highest token id = the EOT token (result read-out, host glue)
         pooled = out[torch.arange(B, device=out.device), ws["ids"].argmax(dim=-1)]

@@ -9,10 +9,9 @@ pooler_output = post_layernorm(last_hidden_state[:, 0]); image_embeds = pooler_o
 Restated in tests/clip_vision_oracle.py and pinned against the installed transformers' CLIPVisionModelWithProjection.
 
 Here: glg_patchify_nchw (14 x 14 stride-14 patches as GEMM rows) + glg_gemm against the repacked conv weight with fp32 out,
-glg_clip_vision_embed (class token, position add and pre_layrnorm in one launch), the blocks as in ClipTextEngine (fused-QKV
-GEMM, the wgmma attention kernel over 257 keys, residual / quick_gelu epilogues), glg_clip_image_head (post_layernorm of the
-class token, visual projection and GLIGEN's reprojection in fp32).  bf16 activations and weights, fp32 accumulation /
-statistics / head, fp32 outputs.
+glg_clip_vision_embed (class token, position add and pre_layrnorm in one launch), the blocks of clip_encoder.py (the wgmma
+attention kernel over 257 keys, no mask), glg_clip_image_head (post_layernorm of the class token, visual projection and
+GLIGEN's reprojection in fp32).  bf16 activations and weights, fp32 accumulation / statistics / head, fp32 outputs.
 """
 from __future__ import annotations
 
@@ -23,7 +22,8 @@ from typing import Dict, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-ACT_QUICK_GELU = 3
+from .clip_encoder import ClipEncoderEngine, layer_param_shapes, synthetic_state_dict
+
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)          # CLIPImageProcessor image_mean / image_std
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
 
@@ -66,42 +66,16 @@ def clip_vision_param_shapes(cfg: ClipVisionConfig, prefix: str = "") -> "Ordere
     p[f"{v}.embeddings.patch_embedding.weight"] = (C, 3, cfg.patch, cfg.patch)
     p[f"{v}.embeddings.position_embedding.weight"] = (cfg.tokens, C)
     p[f"{v}.pre_layrnorm.weight"], p[f"{v}.pre_layrnorm.bias"] = (C,), (C,)
-    for i in range(cfg.layers):
-        l = f"{v}.encoder.layers.{i}"
-        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
-            p[f"{l}.self_attn.{n}.weight"], p[f"{l}.self_attn.{n}.bias"] = (C, C), (C,)
-        p[f"{l}.layer_norm1.weight"], p[f"{l}.layer_norm1.bias"] = (C,), (C,)
-        p[f"{l}.mlp.fc1.weight"], p[f"{l}.mlp.fc1.bias"] = (cfg.ffn, C), (cfg.ffn,)
-        p[f"{l}.mlp.fc2.weight"], p[f"{l}.mlp.fc2.bias"] = (C, cfg.ffn), (C,)
-        p[f"{l}.layer_norm2.weight"], p[f"{l}.layer_norm2.bias"] = (C,), (C,)
+    p.update(layer_param_shapes(cfg, f"{v}."))
     p[f"{v}.post_layernorm.weight"], p[f"{v}.post_layernorm.bias"] = (C,), (C,)
     p[f"{prefix}visual_projection.weight"] = (cfg.projection, C)
     return p
 
 
 def synthetic_clip_vision_state_dict(cfg: ClipVisionConfig, seed: int = 0, prefix: str = "") -> Dict[str, torch.Tensor]:
-    """Seeded fp32 weights, the scheme of clip_text.synthetic_clip_state_dict: projections and the patch convolution ~ N(0, 1/fan_in),
-    class / position embeddings ~ N(0, 0.02) / N(0, 0.01), norm scales 1 + 0.1 N, biases 0.05 N; a few class-embedding channels
-    are scaled up like the massive channels trained CLIP towers show."""
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    sd: Dict[str, torch.Tensor] = OrderedDict()
-    for key, shape in clip_vision_param_shapes(cfg, prefix).items():
-        if key.endswith("class_embedding"):
-            t = torch.randn(shape, generator=g) * 0.02
-            t[:: max(1, cfg.width // 4)] *= 8.0
-        elif key.endswith("position_embedding.weight"):
-            t = torch.randn(shape, generator=g) * 0.01
-        elif key.endswith(".bias"):
-            t = torch.randn(shape, generator=g) * 0.05
-        elif len(shape) == 1:
-            t = 1.0 + 0.1 * torch.randn(shape, generator=g)
-        else:
-            fan_in = 1
-            for s in shape[1:]:
-                fan_in *= s
-            t = torch.randn(shape, generator=g) * (fan_in ** -0.5)
-        sd[key] = t
-    return sd
+    """Seeded fp32 weights, the scheme of clip_encoder.synthetic_state_dict (the patch convolution ~ N(0, 1/fan_in) too); the
+    class embedding carries the scaled-up massive channels."""
+    return synthetic_state_dict(clip_vision_param_shapes(cfg, prefix), seed, massive="class_embedding")
 
 
 def synthetic_pixel_values(N: int, seed: int = 0, size: int = 224) -> torch.Tensor:
@@ -119,20 +93,7 @@ def synthetic_projection_matrix(D: int = 768, seed: int = 0) -> torch.Tensor:
     return torch.randn(D, D, generator=g) * D ** -0.5
 
 
-class ClipVisionEngine:
-    def __init__(self, cfg: ClipVisionConfig, ops):
-        self.cfg, self.ops, self.dev = cfg, ops, ops.device
-        self.adt = ops.act_dtype
-        self.W: Dict[str, torch.Tensor] = {}
-        self._ws: Dict[int, Dict[str, torch.Tensor]] = {}
-        self.loaded = False
-
-    def _a(self, t):
-        return t.detach().to(device=self.dev, dtype=self.adt).contiguous()
-
-    def _f(self, t):
-        return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()
-
+class ClipVisionEngine(ClipEncoderEngine):
     def load_state_dict(self, sd: Dict[str, torch.Tensor]) -> None:
         """Accepts the keys of CLIPModel (`vision_model.*`, `visual_projection.weight`; the text tower's `text_model.*`,
         `text_projection.weight` and `logit_scale` are ignored), of CLIPVisionModelWithProjection (the same two prefixes) or bare
@@ -147,15 +108,7 @@ class ClipVisionEngine:
         w = sd[pre + "embeddings.patch_embedding.weight"].detach().float().permute(0, 2, 3, 1).reshape(C, 3 * k * k)
         W["patch"] = self._a(F.pad(w, (0, cfg.k_pad - 3 * k * k)))
         W["pre.g"], W["pre.b"] = self._f(sd[pre + "pre_layrnorm.weight"]), self._f(sd[pre + "pre_layrnorm.bias"])
-        for i in range(cfg.layers):
-            l = f"{pre}encoder.layers.{i}"
-            W[f"{i}.ln1.g"], W[f"{i}.ln1.b"] = self._f(sd[f"{l}.layer_norm1.weight"]), self._f(sd[f"{l}.layer_norm1.bias"])
-            W[f"{i}.ln2.g"], W[f"{i}.ln2.b"] = self._f(sd[f"{l}.layer_norm2.weight"]), self._f(sd[f"{l}.layer_norm2.bias"])
-            W[f"{i}.qkv.w"] = self._a(torch.cat([sd[f"{l}.self_attn.{n}_proj.weight"] for n in ("q", "k", "v")], dim=0))
-            W[f"{i}.qkv.b"] = self._f(torch.cat([sd[f"{l}.self_attn.{n}_proj.bias"] for n in ("q", "k", "v")], dim=0))
-            W[f"{i}.out.w"], W[f"{i}.out.b"] = self._a(sd[f"{l}.self_attn.out_proj.weight"]), self._f(sd[f"{l}.self_attn.out_proj.bias"])
-            W[f"{i}.fc1.w"], W[f"{i}.fc1.b"] = self._a(sd[f"{l}.mlp.fc1.weight"]), self._f(sd[f"{l}.mlp.fc1.bias"])
-            W[f"{i}.fc2.w"], W[f"{i}.fc2.b"] = self._a(sd[f"{l}.mlp.fc2.weight"]), self._f(sd[f"{l}.mlp.fc2.bias"])
+        self._load_layers(sd, pre)
         W["post.g"], W["post.b"] = self._f(sd[pre + "post_layernorm.weight"]), self._f(sd[pre + "post_layernorm.bias"])
         W["proj"] = self._f(sd[next(k for k in sd if k.endswith("visual_projection.weight"))])
         assert W["proj"].shape == (cfg.projection, C)
@@ -178,20 +131,11 @@ class ClipVisionEngine:
         assert pixel_values.shape == (N, 3, c.image_size, c.image_size), pixel_values.shape
         ws = self._workspace(N)
         ws["px"].copy_(pixel_values)
-        x, t, qkv, ao, h = ws["x"], ws["t"], ws["qkv"], ws["ao"], ws["h"]
-        C, d, T = c.width, c.width // c.heads, c.tokens
         ops.patchify_nchw(ws["px"], ws["pt"], c.image_size, c.image_size, c.patch)
         ops.gemm(ws["pt"], W["patch"], ws["pe"])
-        ops.clip_vision_embed(ws["pe"], W["cls"], W["pos"], W["pre.g"], W["pre.b"], x, c.patches, c.eps)
-        for i in range(c.layers):
-            ops.layernorm_rows(x, t, W[f"{i}.ln1.g"], W[f"{i}.ln1.b"], C, c.eps)
-            ops.gemm(t, W[f"{i}.qkv.w"], qkv.view(N * T, 3 * C), bias=W[f"{i}.qkv.b"])
-            ops.attention(qkv[:, :, :C], qkv[:, :, C: 2 * C], qkv[:, :, 2 * C:], ao, c.heads, d, causal=False)
-            ops.gemm(ao.view(N * T, C), W[f"{i}.out.w"], x, bias=W[f"{i}.out.b"], residual=x)
-            ops.layernorm_rows(x, t, W[f"{i}.ln2.g"], W[f"{i}.ln2.b"], C, c.eps)
-            ops.gemm(t, W[f"{i}.fc1.w"], h, bias=W[f"{i}.fc1.b"], act=ACT_QUICK_GELU)
-            ops.gemm(h, W[f"{i}.fc2.w"], x, bias=W[f"{i}.fc2.b"], residual=x)
-        ops.clip_image_head(x.view(N, T, C), W["post.g"], W["post.b"], W["proj"], ws["pooled"], ws["emb"],
+        ops.clip_vision_embed(ws["pe"], W["cls"], W["pos"], W["pre.g"], W["pre.b"], ws["x"], c.patches, c.eps)
+        self._run_layers(ws, causal=False)
+        ops.clip_image_head(ws["x"].view(N, c.tokens, c.width), W["post.g"], W["post.b"], W["proj"], ws["pooled"], ws["emb"],
                             proj, None if proj is None else ws["feat"], target_norm, c.eps)
         return ws
 

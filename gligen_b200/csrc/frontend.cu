@@ -102,9 +102,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_kernel(const bf16* __restr
       for (int j = 0; j < 8; ++j) s += v[i][j];
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s / (float)C;
+  const float mean = warp_sum(s) / (float)C;
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
@@ -113,9 +111,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_kernel(const bf16* __restr
       for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; q = fmaf(d, d, q); }
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float rstd = rsqrtf(q / (float)C + eps);
+  const float rstd = rsqrtf(warp_sum(q) / (float)C + eps);
 #pragma unroll
   for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
     const int c8 = lane + 32 * i;
@@ -370,9 +366,7 @@ __global__ void __launch_bounds__(256) clip_vision_embed_kernel(const float* __r
       for (int j = 0; j < 8; ++j) s += v[i][j];
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s / (float)C;
+  const float mean = warp_sum(s) / (float)C;
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
@@ -381,9 +375,7 @@ __global__ void __launch_bounds__(256) clip_vision_embed_kernel(const float* __r
       for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; q = fmaf(d, d, q); }
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float rstd = rsqrtf(q / (float)C + eps);
+  const float rstd = rsqrtf(warp_sum(q) / (float)C + eps);
 #pragma unroll
   for (int i = 0; i < LNR_MAX_CHUNKS; ++i) {
     const int c8 = lane + 32 * i;

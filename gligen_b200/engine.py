@@ -19,14 +19,8 @@ from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 
-from .ops import gn_scratch_floats
+from .ops import ACT_SILU, EngineBase, gn_scratch_floats, round_up
 from .spec import UNetConfig, block_schedule
-
-ACT_NONE, ACT_SILU = 0, 1
-
-
-def _rup(x: int, m: int) -> int:
-    return (x + m - 1) // m * m
 
 
 class Plan:
@@ -55,12 +49,10 @@ class Plan:
             fn()
 
 
-class Engine:
+class Engine(EngineBase):
     def __init__(self, cfg: UNetConfig, ops, use_graphs: bool = True):
+        super().__init__(ops)
         self.cfg = cfg
-        self.ops = ops
-        self.dev = ops.device
-        self.adt = ops.act_dtype
         self.blocks = block_schedule(cfg)
         self.W: Dict[str, torch.Tensor] = {}
         self.plans: Dict[Tuple[int, int, int], Plan] = {}
@@ -82,17 +74,11 @@ class Engine:
         self._last_N: Optional[int] = None      # grounding slots of the last grounded call (shape of the null input)
         self._map_shape: Optional[Tuple[int, int, int]] = None    # spatial modalities: (C, H, W) of the conditioning map
         self.n_streams = 2 if cfg.tokenizer == "text_image" else 1
-        self.pos_k = _rup(cfg.tok_feat_dim + cfg.position_dim, 64)
+        self.pos_k = round_up(cfg.tok_feat_dim + cfg.position_dim, 64)
 
     # ------------------------------------------------------------------------------------------
     # weights
     # ------------------------------------------------------------------------------------------
-    def _a(self, t: torch.Tensor) -> torch.Tensor:
-        return t.detach().to(device=self.dev, dtype=self.adt).contiguous()
-
-    def _f(self, t: torch.Tensor) -> torch.Tensor:
-        return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()
-
     @staticmethod
     def _pack_geglu(w: torch.Tensor, *vecs: torch.Tensor):
         """[x rows | gate rows] -> per 256-row tile [128 x | 128 gate] (glg_gemm geglu layout); per-row vectors
@@ -116,12 +102,6 @@ class Engine:
         if bias is not None:
             b = b + bias.float()
         return wf, colsum, b
-
-    @staticmethod
-    def _pack_conv3(w: torch.Tensor) -> torch.Tensor:
-        """[Cout, Cin, 3, 3] -> [9*Cout, Cin] (tap-major)."""
-        co, ci = w.shape[:2]
-        return w.permute(2, 3, 0, 1).reshape(9 * co, ci)
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor]) -> None:
         cfg, W = self.cfg, self.W

@@ -39,6 +39,34 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else t.data_ptr()
 
 
+def round_up(x: int, m: int) -> int:
+    return (x + m - 1) // m * m
+
+
+class EngineBase:
+    """What every engine shares: its ops backend, and weights staged on the ops' device in the activation dtype (`_a`) or in
+    fp32 (`_f`)."""
+
+    def __init__(self, ops):
+        self.ops, self.dev, self.adt = ops, ops.device, ops.act_dtype
+
+    def _a(self, t: torch.Tensor) -> torch.Tensor:
+        return t.detach().to(device=self.dev, dtype=self.adt).contiguous()
+
+    def _f(self, t: torch.Tensor) -> torch.Tensor:
+        return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()
+
+    @staticmethod
+    def _pack_conv3(w: torch.Tensor) -> torch.Tensor:
+        """[Cout, Cin, 3, 3] -> [9*Cout, Cin] (tap-major), the weight of gemm(conv=...)."""
+        co, ci = w.shape[:2]
+        return w.permute(2, 3, 0, 1).reshape(9 * co, ci)
+
+
+# gemm(act=...): the epilogue activation, GLG_ACT_* of include/gligen_b200.h
+ACT_NONE, ACT_SILU, ACT_GELU, ACT_QUICK_GELU = 0, 1, 2, 3
+
+
 class CudaOps:
     """bf16 activations / fp32 statistics on one CUDA device."""
 

@@ -19,14 +19,10 @@ from typing import Dict
 
 import torch
 
+from .ops import ACT_GELU, ACT_SILU, round_up
 from .spec import CONVNEXT_TINY_DEPTHS as DEPTHS, CONVNEXT_TINY_DIMS as DIMS
 
-ACT_NONE, ACT_SILU, ACT_GELU = 0, 1, 2
 _PN, _CX = "position_net", "position_net.convnext_tiny_backbone"
-
-
-def _rup(x: int, m: int) -> int:
-    return (x + m - 1) // m * m
 
 
 def _pad2(w: torch.Tensor, rows: int, cols: int) -> torch.Tensor:
@@ -44,7 +40,7 @@ def _pad1(v: torch.Tensor, n: int) -> torch.Tensor:
 def pack(engine, sd: Dict[str, torch.Tensor]) -> None:
     """ConvNeXt / PositionNet MLP / downsampler weights into the engine's packed table (keys "cx.*", "pn.*", "ds.*")."""
     cfg, W, a, f = engine.cfg, engine.W, engine._a, engine._f
-    cp = [_rup(c, 64) for c in DIMS]                      # 128, 192, 384, 768
+    cp = [round_up(c, 64) for c in DIMS]                  # 128, 192, 384, 768
     d = f"{_CX}.downsample_layers"
     w = sd[f"{d}.0.0.weight"].float()                     # [96, 3, 4, 4] -> [Cout, (ky, kx, c)]
     W["cx.stem.w"] = a(_pad2(w.permute(0, 2, 3, 1).reshape(DIMS[0], -1), cp[0], 64))
@@ -86,7 +82,7 @@ def emit_tokenizer(engine, P, Bt: int, objs: torch.Tensor) -> None:
     """Static plan steps: P.inp["map"] fp32 [Bt, Cm, Hm, Wm], P.inp["gmask"] fp32 [Bt]  ->  objs bf16 [Bt * n, out_dim]."""
     cfg, ops, W = engine.cfg, engine.ops, engine.W
     R, n = cfg.tok_resize, cfg.spatial_tokens
-    cp = [_rup(c, 64) for c in DIMS]
+    cp = [round_up(c, 64) for c in DIMS]
     side = [R // 4, R // 8, R // 16, R // 32]
     rows = [Bt * s * s for s in side]
     xa = engine._buf(max(r * c for r, c in zip(rows, cp)))

@@ -30,15 +30,14 @@ from typing import Dict
 
 import torch
 
+from .ops import EngineBase, gn_scratch_floats
 from .spec import VAEDecoderConfig
 
 
-class _VAEEngineBase:
+class _VAEEngineBase(EngineBase):
     def __init__(self, cfg: VAEDecoderConfig, ops):
+        super().__init__(ops)
         self.cfg = cfg
-        self.ops = ops
-        self.dev = ops.device
-        self.adt = ops.act_dtype
         self.W: Dict[str, torch.Tensor] = {}
         self.loaded = False
         chans = [cfg.ch * m for m in cfg.ch_mult]
@@ -46,17 +45,6 @@ class _VAEEngineBase:
             raise ValueError(f"VAE channels {chans} must be multiples of 64 for the tensor-core tiles")
 
     # ---- weights ---------------------------------------------------------------------------------------------
-    def _a(self, t):
-        return t.detach().to(device=self.dev, dtype=self.adt).contiguous()
-
-    def _f(self, t):
-        return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()
-
-    @staticmethod
-    def _pack_conv3(w):
-        co, ci = w.shape[:2]
-        return w.permute(2, 3, 0, 1).reshape(9 * co, ci)          # [9*Cout, Cin], tap-major
-
     def _load_res(self, sd, prefix):
         W = self.W
         for n in ("norm1", "norm2"):
@@ -158,7 +146,6 @@ class VAEDecoderEngine(_VAEEngineBase):
         """z: fp32 [B, embed_dim, h, w] (the sampler's latent) -> image fp32 [B, out_ch, 8h, 8w] (for 4 levels)."""
         assert self.loaded, "load_state_dict first"
         cfg, ops, W = self.cfg, self.ops, self.W
-        from .ops import gn_scratch_floats
         B, _, H, Wd = z.shape
         assert H == Wd, "square latents only"
         z = z.to(device=self.dev, dtype=torch.float32).contiguous()
@@ -222,7 +209,6 @@ class VAEEncoderEngine(_VAEEngineBase):
         """x: fp32 image [B, in_channels, S, S] -> moments fp32 [B, 2 * embed_dim, S / 2^(levels-1), ...]."""
         assert self.loaded, "load_state_dict first"
         cfg, ops, W = self.cfg, self.ops, self.W
-        from .ops import gn_scratch_floats
         B, Cin, H, Wd = x.shape
         nlev = len(cfg.ch_mult)
         assert H == Wd and Cin == cfg.in_channels and H % (1 << (nlev - 1)) == 0, "square images, side a multiple of 2^(levels-1)"

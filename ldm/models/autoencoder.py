@@ -17,6 +17,7 @@ import torch.nn as nn
 
 from gligen_b200 import _overlay
 from gligen_b200.spec import VAEDecoderConfig, vae_decoder_param_shapes, vae_encoder_param_shapes
+from ldm.modules.attention import attach_params
 
 _ref = _overlay._shadowed_module(__name__, __file__)
 
@@ -113,9 +114,6 @@ if _ref is not None:
                 return _ref.AutoencoderKL.encode(self, x)
             return _CudaDecodeMixin.encode(self, x)
 else:
-    class _Node(nn.Module):
-        pass
-
     class AutoencoderKL(_CudaDecodeMixin, nn.Module):
         """Parameters under the reference's names (no reference checkout behind this repo); compute is CUDA only."""
 
@@ -126,14 +124,7 @@ else:
             self._glg_cfg = _cfg_from_ddconfig(ddconfig, embed_dim, scale_factor)
             shapes = dict(vae_encoder_param_shapes(self._glg_cfg))
             shapes.update(vae_decoder_param_shapes(self._glg_cfg))
-            for key, shape in shapes.items():
-                node = self
-                parts = key.split(".")
-                for name in parts[:-1]:
-                    if name not in node._modules:
-                        node.add_module(name, _Node())
-                    node = node._modules[name]
-                node.register_parameter(parts[-1], nn.Parameter(torch.zeros(shape), requires_grad=False))
+            attach_params(self, shapes, "")
             self._glg_engine, self._glg_stale = None, True
 
         def post_quant_conv_weight_device(self):

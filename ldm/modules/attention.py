@@ -30,6 +30,20 @@ class ParamNode(nn.Module):
                            "(the whole denoiser runs inside the gligen_b200 engine)")
 
 
+def attach_params(root: ParamNode, shapes, strip: str, node_cls=lambda path: ParamNode):
+    """Create nested ParamNodes + zero-initialised fp32 parameters for every `strip`-prefixed key."""
+    for key, shape in shapes.items():
+        if not key.startswith(strip):
+            continue
+        parts = key[len(strip):].split(".")
+        node = root
+        for i, name in enumerate(parts[:-1]):
+            if name not in node._modules:
+                node.add_module(name, node_cls(".".join(parts[: i + 1]))())
+            node = node._modules[name]
+        node.register_parameter(parts[-1], nn.Parameter(torch.zeros(shape), requires_grad=False))
+
+
 class LinearAttention(nn.Module):
     """Softmax-over-keys linear attention on feature maps (reference attention.py:80-99).  NOT on the denoiser's path
     (no UNet config uses it); it lives here, as ordinary PyTorch, only because the reference's VAE module

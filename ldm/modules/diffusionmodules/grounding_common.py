@@ -1,11 +1,8 @@
 """Shared constructor logic of the PositionNet / GroundingDownsampler containers (parameters only)."""
 from dataclasses import replace
 
-import torch
-import torch.nn as nn
-
 from gligen_b200.spec import SPATIAL_TOKENIZERS, UNetConfig, downsampler_param_shapes, unet_param_shapes
-from ldm.modules.attention import ParamNode
+from ldm.modules.attention import ParamNode, attach_params
 
 
 def tokenizer_config(kind: str, base: UNetConfig = UNetConfig(), **params) -> UNetConfig:
@@ -17,20 +14,6 @@ def tokenizer_config(kind: str, base: UNetConfig = UNetConfig(), **params) -> UN
                        tok_out_dim=params.get("out_dim", 768), fourier_freqs=params.get("fourier_freqs", 8))
     return replace(base, tokenizer=kind, tok_in_dim=params.get("in_dim", 768), tok_out_dim=params.get("out_dim", 768),
                    fourier_freqs=params.get("fourier_freqs", 8))
-
-
-def attach_params(root: ParamNode, shapes, strip: str, node_cls=lambda path: ParamNode):
-    """Create nested ParamNodes + zero-initialised fp32 parameters for every `strip`-prefixed key."""
-    for key, shape in shapes.items():
-        if not key.startswith(strip):
-            continue
-        parts = key[len(strip):].split(".")
-        node = root
-        for i, name in enumerate(parts[:-1]):
-            if name not in node._modules:
-                node.add_module(name, node_cls(".".join(parts[: i + 1]))())
-            node = node._modules[name]
-        node.register_parameter(parts[-1], nn.Parameter(torch.zeros(shape), requires_grad=False))
 
 
 def downsampler_config(kind: str, base: UNetConfig, **params) -> UNetConfig:

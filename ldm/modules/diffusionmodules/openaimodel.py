@@ -16,9 +16,9 @@ import torch.nn as nn
 
 from gligen_b200.spec import UNetConfig, unet_param_shapes
 from ldm.modules.attention import (BasicTransformerBlock, CrossAttention, FeedForward, GatedSelfAttentionDense,
-                                   ParamNode, SelfAttention, SpatialTransformer)
+                                   ParamNode, SelfAttention, SpatialTransformer, attach_params)
 from gligen_b200.spec import SPATIAL_TOKENIZERS
-from ldm.modules.diffusionmodules.grounding_common import attach_params, downsampler_config, tokenizer_config
+from ldm.modules.diffusionmodules.grounding_common import downsampler_config, tokenizer_config
 from ldm.util import instantiate_from_config
 
 _TOKENIZERS = {

@@ -16,15 +16,12 @@ import torch.nn as nn
 
 from gligen_b200 import _overlay
 from gligen_b200.clip_text import SD14_CLIP_TEXT, ClipTextConfig, ClipTextEngine, clip_text_param_shapes
+from ldm.modules.attention import attach_params
 
 
 class AbstractEncoder(nn.Module):
     def encode(self, *args, **kwargs):
         raise NotImplementedError
-
-
-class _Node(nn.Module):
-    pass
 
 
 class FrozenCLIPEmbedder(AbstractEncoder):
@@ -42,14 +39,7 @@ class FrozenCLIPEmbedder(AbstractEncoder):
             text_config = ClipTextConfig(**text_config)
         self.cfg = text_config or SD14_CLIP_TEXT
         self._tokenizer = None
-        for key, shape in clip_text_param_shapes(self.cfg, "transformer.").items():
-            node = self
-            parts = key.split(".")
-            for name in parts[:-1]:
-                if name not in node._modules:
-                    node.add_module(name, _Node())
-                node = node._modules[name]
-            node.register_parameter(parts[-1], nn.Parameter(torch.zeros(shape), requires_grad=False))
+        attach_params(self, clip_text_param_shapes(self.cfg, "transformer."), "")
         self._engine, self._stale = None, True
 
     # ---- weights ----------------------------------------------------------------------------------------------------

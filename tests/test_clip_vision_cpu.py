@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from clip_vision_oracle import clip_vision_forward, gligen_image_feature, prepare_batch as oracle_prepare_batch
-from clip_vision_ref_ops import ClipVisionRefOps as RefOps
+from ref_ops import RefOps
 from conftest import GOLD
 from gligen_b200.clip_text import TINY_CLIP_TEXT, synthetic_clip_state_dict, synthetic_token_ids
 from gligen_b200.clip_vision import (NAMED_CLIP_VISION_CONFIGS, TINY_CLIP_VISION, ClipVisionEngine, clip_vision_param_shapes,

@@ -49,7 +49,7 @@ def test_clip_vision_embed_within_one_ulp(ops, N, C, ratio):
     so the only fp32 error left before the bf16 rounding is that of rstd (sum of C squares, rsqrtf), which scales with the
     normalised term |gamma (x - mean) rstd|.  Bound per element: one bf16 ulp of the rounded float64 result plus
     (C / 2 + 8) 2^-24 of that term (the term is beta-cancelled near zero, where one ulp alone would be below fp32 round-off)."""
-    from clip_vision_ref_ops import ClipVisionRefOps as RefOps
+    from ref_ops import RefOps
     P = 256
     g = gen(C + N)
     q = lambda t: torch.round(t * 64) / 64
