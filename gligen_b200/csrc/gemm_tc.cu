@@ -10,7 +10,17 @@
 //                   (LayerNorm fold / bias / time-embedding row bias / SiLU / GELU / tanh-gate / residual / GEGLU ->
 //                   bf16 or fp32 global stores, per-row LayerNorm partial sums of what is stored)
 //
-// Two instantiations of the same code:
+// Two consumer schedules:
+//   PP = false (cooperative): both consumer warpgroups share one 128 x BN work item, 64 rows each, and run its epilogue
+//                  together while the tensor pipe idles.
+//   PP = true  (ping-pong): each consumer warpgroup owns whole 128 x BN work items (two m64 x BN accumulators, rows 0-63 and
+//                  64-127 of the same A stage): warpgroup 0 takes the CTA's even items, warpgroup 1 the odd ones.  An MMA
+//                  token passed through two named barriers lets only one of them issue wgmmas at a time, so one warpgroup's
+//                  epilogue runs under the other's mainloop.  The producer feeds both through the same in-order ring; each
+//                  warpgroup steps its ring position over the stages of the other's items.  GEGLU items are 128 packed weight
+//                  rows [64 x | 64 gate] cut from the 256-row [128 x | 128 gate] layout: B is staged as two 64-row boxes.
+//
+// Two cluster shapes of the same code:
 //   CTA2 = false : one CTA per 128 x BN tile.
 //   CTA2 = true  : a cluster of two CTAs per 256 x BN tile: each CTA stages its own 128 rows of A and loads HALF of the
 //                  B tile with a TMA multicast into both CTAs, so every weight byte fetched from L2 feeds two CTAs.
@@ -77,8 +87,13 @@ template <int BN, bool CTA2> struct GemmCfg {
 
 __device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+// named barriers 1 / 2 (0 is __syncthreads): the ping-pong MMA token of consumer warpgroup 0 / 1, 256 threads each
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
 
-__device__ __forceinline__ void add2(float& a, float& b, const float* p) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); a += t.x; b += t.y; }
+// GEGLU: first packed weight row of the x half of n-tile n_blk of width BN (the gate rows follow 128 rows later).
+// BN = 256 is one whole [128 x | 128 gate] block; BN = 128 is the upper or lower 64 x rows of one.
+template <int BN> __device__ __forceinline__ int geglu_xrow(int n_blk) { return (n_blk * BN / 256) * 256 + (n_blk * (BN / 2)) % 128; }
 
 __device__ __forceinline__ float act_f(int act, float v) {
   if (act == GLG_ACT_SILU) return silu_f(v);
@@ -90,44 +105,89 @@ __device__ __forceinline__ float act_f(int act, float v) {
 // ---- epilogue of one 64-row x BN accumulator held by a consumer warpgroup ---------------------------------------
 // wgmma m64nN D fragment: warp w of the warpgroup holds rows 16 w + lane / 4 (regs 4 j + 0, 1) and + 8 (regs 4 j + 2, 3),
 // columns 8 j + 2 (lane % 4) + {0, 1}, for j = 0 .. N / 8 - 1.
+// The epilogue walks 32-column chunks and issues every global load of a chunk (bias, LayerNorm column sums, row bias,
+// residual; both rows of the thread) before the chunk's first store: the compiler cannot move a load across a store that
+// may alias it, so loads interleaved with stores would cost one L2 round trip per 8 columns.
 template <int BN, bool GEGLU>
 __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float (&d)[BN / 2], int row_base, int n_blk, float gate, int lane) {
   const int cq = 2 * (lane & 3);
+  int row[2]; bool row_ok[2]; size_t out_off[2];
+  float ln_rstd[2] = {1.f, 1.f}, c1[2] = {0.f, 0.f};     // LayerNorm fold: rstd * acc + (bias - rstd * mu * colsum)
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
-    const int row = row_base + hr * 8;
-    const bool row_ok = row < p.M;
-    float ln_mu = 0.f, ln_rstd = 1.f;
-    if (p.ln_stats && row_ok) {
-      const float2* sp = reinterpret_cast<const float2*>(p.ln_stats) + row;
-      float s1 = 0.f, s2 = 0.f;
-      for (int i = 0; i < p.ln_slots; ++i) { const float2 t = __ldg(sp + (size_t)i * p.ln_stride); s1 += t.x; s2 += t.y; }   // fixed order
-      ln_mu = s1 * p.inv_k;
-      ln_rstd = rsqrtf(fmaxf(s2 * p.inv_k - ln_mu * ln_mu, 0.f) + p.ln_eps);
+    row[hr] = row_base + hr * 8;
+    row_ok[hr] = row[hr] < p.M;
+    out_off[hr] = p.orpb ? (size_t)(row[hr] / p.orpb) * p.obs + (size_t)(row[hr] % p.orpb) * p.ldc : (size_t)row[hr] * p.ldc;
+  }
+  if (p.ln_stats) {
+    const float2* sp = reinterpret_cast<const float2*>(p.ln_stats);
+    const int r0 = row_ok[0] ? row[0] : 0, r1 = row_ok[1] ? row[1] : 0;
+    float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+    for (int i = 0; i < p.ln_slots; ++i) {                 // fixed order
+      const float2 t0 = __ldg(sp + (size_t)i * p.ln_stride + r0), t1 = __ldg(sp + (size_t)i * p.ln_stride + r1);
+      s1[0] += t0.x; s2[0] += t0.y; s1[1] += t1.x; s2[1] += t1.y;
     }
-    const float c1 = -ln_rstd * ln_mu;              // LayerNorm fold: rstd * acc + (bias - rstd * mu * colsum)
-    const size_t out_off = p.orpb ? (size_t)(row / p.orpb) * p.obs + (size_t)(row % p.orpb) * p.ldc : (size_t)row * p.ldc;
-    if constexpr (GEGLU) {
-      constexpr int HALF = BN / 2;                  // packed weight rows per tile: [128 x | 128 gate]
 #pragma unroll
-      for (int j = 0; j < HALF / 8; ++j) {
-        const int c = 8 * j + cq;
-        const int wcol = n_blk * BN + c;
-        float bx0 = __ldg(p.bias + wcol), bx1 = __ldg(p.bias + wcol + 1);
-        float bg0 = __ldg(p.bias + wcol + HALF), bg1 = __ldg(p.bias + wcol + HALF + 1);
+    for (int hr = 0; hr < 2; ++hr) {
+      const float mu = s1[hr] * p.inv_k;
+      ln_rstd[hr] = rsqrtf(fmaxf(s2[hr] * p.inv_k - mu * mu, 0.f) + p.ln_eps);
+      c1[hr] = -ln_rstd[hr] * mu;
+    }
+  }
+  if constexpr (GEGLU) {
+    constexpr int HALF = BN / 2;                    // tile columns [HALF x | HALF gate], packed weight rows x and x + 128
+    const int xrow = geglu_xrow<BN>(n_blk);
+#pragma unroll
+    for (int ch = 0; ch < HALF / 32; ++ch) {
+      float2 bx[4], bg[4], cx[4], cg[4];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int wcol = xrow + 32 * ch + 8 * jj + cq;
+        bx[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + wcol));
+        bg[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + wcol + 128));
         if (p.ln_stats) {
-          bx0 = fmaf(__ldg(p.ln_colsum + wcol), c1, bx0); bx1 = fmaf(__ldg(p.ln_colsum + wcol + 1), c1, bx1);
-          bg0 = fmaf(__ldg(p.ln_colsum + wcol + HALF), c1, bg0); bg1 = fmaf(__ldg(p.ln_colsum + wcol + HALF + 1), c1, bg1);
+          cx[jj] = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + wcol));
+          cg[jj] = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + wcol + 128));
         }
-        const float x0 = fmaf(d[4 * j + 2 * hr], ln_rstd, bx0), x1 = fmaf(d[4 * j + 2 * hr + 1], ln_rstd, bx1);
-        const float g0 = fmaf(d[HALF / 2 + 4 * j + 2 * hr], ln_rstd, bg0), g1 = fmaf(d[HALF / 2 + 4 * j + 2 * hr + 1], ln_rstd, bg1);
-        if (row_ok)
-          *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + out_off + n_blk * HALF + c) = pack_bf16x2(geglu_f(x0, g0), geglu_f(x1, g1));
       }
-    } else {
-      const float* rb = (p.rowbias && row_ok) ? p.rowbias + (size_t)(row / p.rows_per_batch) * p.ld_rowbias : nullptr;
 #pragma unroll
-      for (int ch = 0; ch < BN / 32; ++ch) {        // 32-column chunks: one LayerNorm-statistics slot each
+      for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * ch + jj;
+          float bx0 = bx[jj].x, bx1 = bx[jj].y, bg0 = bg[jj].x, bg1 = bg[jj].y;
+          if (p.ln_stats) {
+            bx0 = fmaf(cx[jj].x, c1[hr], bx0); bx1 = fmaf(cx[jj].y, c1[hr], bx1);
+            bg0 = fmaf(cg[jj].x, c1[hr], bg0); bg1 = fmaf(cg[jj].y, c1[hr], bg1);
+          }
+          const float x0 = fmaf(d[4 * j + 2 * hr], ln_rstd[hr], bx0), x1 = fmaf(d[4 * j + 2 * hr + 1], ln_rstd[hr], bx1);
+          const float g0 = fmaf(d[HALF / 2 + 4 * j + 2 * hr], ln_rstd[hr], bg0), g1 = fmaf(d[HALF / 2 + 4 * j + 2 * hr + 1], ln_rstd[hr], bg1);
+          if (row_ok[hr])
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + out_off[hr] + n_blk * HALF + 8 * j + cq) = pack_bf16x2(geglu_f(x0, g0), geglu_f(x1, g1));
+        }
+      }
+    }
+  } else {
+    const float* rb[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) rb[hr] = (p.rowbias && row_ok[hr]) ? p.rowbias + (size_t)(row[hr] / p.rows_per_batch) * p.ld_rowbias : nullptr;
+#pragma unroll
+    for (int ch = 0; ch < BN / 32; ++ch) {          // 32-column chunks: one LayerNorm-statistics slot each
+      float2 bias[4], cs[4], rbv[2][4];
+      uint32_t res[2][4];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int n0 = n_blk * BN + 32 * ch + 8 * jj + cq;
+        bias[jj] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0)) : make_float2(0.f, 0.f);
+        if (p.ln_stats) cs[jj] = __ldg(reinterpret_cast<const float2*>(p.ln_colsum + n0));
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          if (rb[hr]) rbv[hr][jj] = __ldg(reinterpret_cast<const float2*>(rb[hr] + n0));
+          if (p.residual && row_ok[hr]) res[hr][jj] = __ldg(reinterpret_cast<const unsigned int*>(p.residual + (size_t)row[hr] * p.ldr + n0));
+        }
+      }
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
         float st_sum = 0.f, st_sq = 0.f;
 #pragma unroll
         for (int jj = 0; jj < 4; ++jj) {
@@ -135,23 +195,21 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float (&d)[B
           const int n0 = n_blk * BN + 8 * j + cq;
           float v0 = d[4 * j + 2 * hr], v1 = d[4 * j + 2 * hr + 1];
           if (p.ln_stats) {
-            float b0 = 0.f, b1 = 0.f;
-            if (p.bias) { b0 = __ldg(p.bias + n0); b1 = __ldg(p.bias + n0 + 1); }
-            v0 = fmaf(v0, ln_rstd, fmaf(__ldg(p.ln_colsum + n0), c1, b0));
-            v1 = fmaf(v1, ln_rstd, fmaf(__ldg(p.ln_colsum + n0 + 1), c1, b1));
-          } else if (p.bias) add2(v0, v1, p.bias + n0);
-          if (rb) add2(v0, v1, rb + n0);
+            v0 = fmaf(v0, ln_rstd[hr], fmaf(cs[jj].x, c1[hr], bias[jj].x));
+            v1 = fmaf(v1, ln_rstd[hr], fmaf(cs[jj].y, c1[hr], bias[jj].y));
+          } else if (p.bias) { v0 += bias[jj].x; v1 += bias[jj].y; }
+          if (rb[hr]) { v0 += rbv[hr][jj].x; v1 += rbv[hr][jj].y; }
           v0 = act_f(p.act, v0); v1 = act_f(p.act, v1);
           if (p.gate) { v0 *= gate; v1 *= gate; }
-          if (p.residual && row_ok) {
-            const float2 r = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(p.residual + (size_t)row * p.ldr + n0)));
+          if (p.residual && row_ok[hr]) {
+            const float2 r = unpack_bf16x2(res[hr][jj]);
             v0 += r.x; v1 += r.y;
           }
           if (p.out_fp32) {
-            if (row_ok) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + out_off + n0) = make_float2(v0, v1);
+            if (row_ok[hr]) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + out_off[hr] + n0) = make_float2(v0, v1);
           } else {
             const uint32_t pk = pack_bf16x2(v0, v1);
-            if (row_ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + out_off + n0) = pk;
+            if (row_ok[hr]) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + out_off[hr] + n0) = pk;
             // statistics of the values AS STORED (bf16-rounded): exactly what the consumer GEMM reads
             const float2 f = unpack_bf16x2(pk);
             st_sum += f.x + f.y;
@@ -164,8 +222,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float (&d)[B
           // a fixed butterfly order.
           st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 1); st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 1);
           st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 2); st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 2);
-          if ((lane & 3) == 0 && row_ok)
-            reinterpret_cast<float2*>(p.stats_out)[(size_t)((n_blk * BN >> 5) + ch) * p.stats_stride + row] = make_float2(st_sum, st_sq);
+          if ((lane & 3) == 0 && row_ok[hr])
+            reinterpret_cast<float2*>(p.stats_out)[(size_t)((n_blk * BN >> 5) + ch) * p.stats_stride + row[hr]] = make_float2(st_sum, st_sq);
         }
       }
     }
@@ -230,12 +288,13 @@ __global__ void splitk_reduce_kernel(const GemmKParams p) {
   }
 }
 
-template <int BN, bool GEGLU, bool CTA2>
+template <int BN, bool GEGLU, bool CTA2, bool PP>
 __global__ void __launch_bounds__(384, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
   using Cfg = GemmCfg<BN, CTA2>;
   constexpr int MAXST = Cfg::MAX_STAGES;
   constexpr int ROWS_PER_TILE = CTA2 ? 256 : 128;
+  constexpr bool B_SPLIT = GEGLU && PP;                               // B staged as two BN/2-row boxes (x rows, gate rows)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t bar_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t base = bar_base + Cfg::BAR_BYTES;                   // tiles (1024-byte aligned)
@@ -246,6 +305,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (MAXST + s); };
   const uint32_t bfull_bar = bar_base + 8u * (2 * MAXST);
+  // first weight row of half q (BN/2 rows) of the B tile of n-tile n_blk
+  auto b_row = [&](int n_blk, int q) { return B_SPLIT ? geglu_xrow<BN>(n_blk) + q * 128 : n_blk * BN + q * (BN / 2); };
 
   pdl_trigger();          // the next kernel may start its prologue while this one runs (it waits before touching memory)
   const int warp = threadIdx.x >> 5;
@@ -256,8 +317,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int num_units = CTA2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    // a stage is free again when every consumer warp (8 per CTA) of every CTA that receives it has released it
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CTA2 ? 16 : 8); }
+    // a stage is free again when every consumer warp that reads it (8 per CTA; ping-pong: the 4 of the owning warpgroup)
+    // of every CTA that receives it has released it
+    constexpr uint32_t releasers = (PP ? 4 : 8) * (CTA2 ? 2 : 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), releasers); }
     mbar_init(bfull_bar, 1);
     fence_barrier_init();
   }
@@ -292,9 +355,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int stage = 0; uint32_t phase = 0;
       if (bres && leader) {
         // the CTA's weight tile, once: num_kb boxes of [BN rows x 64 columns] on one barrier
-        const int brow = (unit % p.tiles_n) * BN;
+        const int nblk = unit % p.tiles_n;
         mbar_arrive_expect_tx(bfull_bar, (uint32_t)p.num_kb * Cfg::B_BYTES);
-        for (int kb = 0; kb < p.num_kb; ++kb) tma_load_2d(bres_base + (uint32_t)kb * Cfg::B_BYTES, &tmB, bfull_bar, kb * 64, brow);
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          const uint32_t dst = bres_base + (uint32_t)kb * Cfg::B_BYTES;
+          tma_load_2d(dst, &tmB, bfull_bar, kb * 64, b_row(nblk, 0));
+          if constexpr (B_SPLIT) tma_load_2d(dst + Cfg::B_HALF, &tmB, bfull_bar, kb * 64, b_row(nblk, 1));
+        }
       }
       int tile, split, m_blk, n_blk;
       for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
@@ -306,7 +373,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           y0 = (row0 - b0 * p.HW) / p.Wd;
           x0 = row0 - b0 * p.HW - y0 * p.Wd;          // non-zero only for images wider than a tile (W > 128: part of one row)
         }
-        const int brow0 = n_blk * BN;
         // K steps are visited in a per-tile rotated order: tiles running at the same time would otherwise request
         // the very same weight (and activation) lines from L2 in lockstep; the rotation spreads them over slices.
         // (fp32 accumulation order depends only on the tile index -> results stay reproducible.)  B-resident tiles
@@ -318,20 +384,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const uint32_t b_dst = a_dst + Cfg::A_BYTES;
           if (leader) {
             mbar_arrive_expect_tx(full_bar(stage), bres ? Cfg::A_BYTES : Cfg::STAGE_BYTES);
-            int ca = kb * 64, cb_row = brow0;
+            int ca = kb * 64, cb_off = 0;
             if (p.conv) {
               const int tap = kb / p.kb_per_tap;
               const int cb = kb - tap * p.kb_per_tap;
               const int dy = tap / 3 - 1, dx = tap - (tap / 3) * 3 - 1;
               tma_load_4d(a_dst, &tmA, full_bar(stage), cb * 64, x0 + dx, y0 + dy, b0);
-              ca = cb * 64; cb_row = tap * p.N + brow0;
+              ca = cb * 64; cb_off = tap * p.N;
             } else {
               tma_load_2d(a_dst, &tmA, full_bar(stage), kb * 64, row0);
             }
             if constexpr (CTA2) {
-              tma_load_2d_mc(b_dst + rank * Cfg::B_HALF, &tmB, full_bar(stage), ca, cb_row + (int)rank * (BN / 2), (uint16_t)3);
+              tma_load_2d_mc(b_dst + rank * Cfg::B_HALF, &tmB, full_bar(stage), ca, cb_off + b_row(n_blk, (int)rank), (uint16_t)3);
             } else if (!bres) {
-              tma_load_2d(b_dst, &tmB, full_bar(stage), ca, cb_row);
+              if constexpr (B_SPLIT) {
+                tma_load_2d(b_dst, &tmB, full_bar(stage), ca, cb_off + b_row(n_blk, 0));
+                tma_load_2d(b_dst + Cfg::B_HALF, &tmB, full_bar(stage), ca, cb_off + b_row(n_blk, 1));
+              } else {
+                tma_load_2d(b_dst, &tmB, full_bar(stage), ca, cb_off + n_blk * BN);
+              }
             }
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
@@ -339,9 +410,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   } else {
-    // ===================== consumers: warpgroup 1 / 2 own accumulator rows [0, 64) / [64, 128) of the tile ==========
+    // ===================== consumers =====================
+    // cooperative: warpgroup 1 / 2 own accumulator rows [0, 64) / [64, 128) of every item;
+    // ping-pong: warpgroup 1 / 2 own the even / odd items of this CTA, all 128 rows (accumulator halves d[0], d[1])
     setmaxnreg_inc232();
     const int cw = wg - 1;
+    constexpr int MH = PP ? 2 : 1;
     const float gate = p.gate ? __ldg(p.gate) : 1.0f;
     uint32_t empty0 = empty_bar(0), empty0_peer = 0;
     if constexpr (CTA2) empty0_peer = mapa_cluster(empty_bar(0), rank ^ 1u);
@@ -353,34 +427,52 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if constexpr (CTA2) mbar_arrive_cluster(empty0_peer + 8u * s);
       }
     };
-    float d[BN / 2];
+    float d[MH][BN / 2];
     int tile, split, m_blk, n_blk;
     for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
       const int kb_n = ((split + 1) * p.num_kb) / p.splits - (split * p.num_kb) / p.splits;
+      if (PP && (it & 1) != cw) {                // the other warpgroup's item: step over its stages
+        stage += kb_n;
+        while (stage >= STAGES) { stage -= STAGES; phase ^= 1u; }
+        continue;
+      }
+      if (PP && it > 0) named_bar_sync(1 + cw);  // the MMA token, passed on by the owner of item it - 1
       int prev = -1;
       for (int kb = 0; kb < kb_n; ++kb) {
         mbar_wait<false>(full_bar(stage), phase);
-        const uint32_t a_addr = base + stage * stage_bytes + (uint32_t)cw * (64 * 128);
-        const uint64_t adesc = gmma_desc_kmajor_sw128(a_addr);
+        const uint32_t a_addr = base + stage * stage_bytes + (uint32_t)(PP ? 0 : cw) * (64 * 128);
         const uint64_t bdesc = gmma_desc_kmajor_sw128(bres ? bres_base + (uint32_t)kb * Cfg::B_BYTES : base + stage * stage_bytes + Cfg::A_BYTES);
-        wgmma_fence_regs(d);
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) wgmma_fence_regs(d[mh]);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)      // 4 x K=16 inside one 64-wide (128 B) swizzle atom: +32 B per step
-          Wgmma<BN>::mma(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1 : 0);
+        for (int k = 0; k < 4; ++k) {    // 4 x K=16 inside one 64-wide (128 B) swizzle atom: +32 B per step
+#pragma unroll
+          for (int mh = 0; mh < MH; ++mh)
+            Wgmma<BN>::mma(d[mh], gmma_desc_kmajor_sw128(a_addr + (uint32_t)mh * (64 * 128)) + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1 : 0);
+        }
         wgmma_commit();
         wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its buffers back to the producer
-        wgmma_fence_regs(d);
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) wgmma_fence_regs(d[mh]);
         if (prev >= 0) release(prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
+      if constexpr (PP) {                        // all MMAs of this item are issued: pass the token to the next item's owner
+        int t2, s2, m2, n2;
+        if (get_work(it + 1, t2, s2, m2, n2)) named_bar_arrive(2 - cw);
+      }
       wgmma_wait<0>();
-      wgmma_fence_regs(d);
+#pragma unroll
+      for (int mh = 0; mh < MH; ++mh) wgmma_fence_regs(d[mh]);
       if (prev >= 0) release(prev);
-      const int row_base = m_blk * ROWS_PER_TILE + (int)rank * 128 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
-      if (p.splits > 1) epilogue_partial<BN>(p, d, row_base, n_blk, split, lane);
-      else epilogue_tile<BN, GEGLU>(p, d, row_base, n_blk, gate, lane);
+#pragma unroll
+      for (int mh = 0; mh < MH; ++mh) {
+        const int row_base = m_blk * ROWS_PER_TILE + (int)rank * 128 + (PP ? mh : cw) * 64 + (warp & 3) * 16 + (lane >> 2);
+        if (p.splits > 1) epilogue_partial<BN>(p, d[mh], row_base, n_blk, split, lane);
+        else epilogue_tile<BN, GEGLU>(p, d[mh], row_base, n_blk, gate, lane);
+      }
     }
   }
   // no CTA of a pair may exit while its peer can still multicast into its smem or arrive on its barriers
@@ -390,11 +482,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // ------------------------------------------------------------------------------------------------
 // launch
 // ------------------------------------------------------------------------------------------------
-template <int BN, bool GEGLU, bool CTA2>
+template <int BN, bool GEGLU, bool CTA2, bool PP>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, size_t smem, cudaStream_t st) {
   using Cfg = GemmCfg<BN, CTA2>;
   static bool attr_set = false;
-  auto kern = gemm_tc_kernel<BN, GEGLU, CTA2>;
+  auto kern = gemm_tc_kernel<BN, GEGLU, CTA2, PP>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_MAX);
     if (e != cudaSuccess) return set_error(std::string("cudaFuncSetAttribute(gemm): ") + cudaGetErrorString(e));
@@ -430,6 +522,7 @@ int g_force_bn = 0;     // test hooks (glg_debug_force_bn / glg_debug_gemm_cta2 
 int g_splitk_mode = 0;  // 0 = heuristic, 1 = never, 2 = split whenever legal
 int g_cta2_mode = -1;   // 0 = heuristic, 1 = never pair, 2 = pair whenever legal; -1 = read GLG_GEMM_CTA2 (default 0)
 int g_bres_mode = -1;   // B-resident tiles: 0 = heuristic, 1 = never, 2 = whenever legal; -1 = read GLG_GEMM_BRES (default 1)
+int g_pp_mode = 0;      // ping-pong consumers (glg_debug_gemm_pp): 0 = heuristic, 1 = never, 2 = whenever legal
 
 static constexpr long long kTileMax = 227 * 1024 - 1024 - 1024;     // dynamic smem minus alignment slack and barriers
 
@@ -445,8 +538,15 @@ static int bres_stages(int bn, int num_kb) {
 //   per 64-wide K step an SM needs max(MMA = 4*BN: 128 x BN x 64 MACs at 2048 bf16 MAC/clk, operand bytes / ~32 B/clk of
 //   L2->SM bandwidth) cycles (a pair stages 128 + BN/2 operand rows per SM instead of 128 + BN); a CTA pays ~3000 cycles
 //   of fixed cost per work item; split-K adds a reduce pass over splits * M * N fp32.  The least estimated time wins.
+// Schedule: ping-pong only where a forced-tile sweep (scripts/sweep_bn.py, H100 80GB HBM3 at 400 W) measured it ahead of
+// every cooperative tile: 3x3 convolutions with M >= 8192 on 64-wide tiles (SD levels 0-1 at 8 rows: 0.72-0.87x the
+// time of the cooperative tile the model picks) and GEGLU with M <= 512 (0.87x).  Elsewhere it measured level or slower.
+static bool pingpong_pays(int M, int bn, bool geglu, bool conv) {
+  return (conv && M >= 8192 && bn == 64) || (geglu && M <= 512);
+}
+
 static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_splits, long long ws_bytes,
-                      int* bn_out, int* cta2_out, int* splits_out, int* bres_out) {
+                      int* bn_out, int* cta2_out, int* splits_out, int* bres_out, int* pp_out) {
   if (g_cta2_mode < 0) {
     const char* e = getenv("GLG_GEMM_CTA2");
     g_cta2_mode = e ? atoi(e) : 0;
@@ -457,7 +557,7 @@ static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_s
   }
   const int sms = num_sms();
   const int cands[4] = {256, 160, 128, 64};
-  float best = 1e30f; int best_bn = 0, best_pair = 0, best_s = 1, best_res = 0;
+  float best = 1e30f; int best_bn = 0, best_pair = 0, best_s = 1, best_res = 0, best_pp = 0;
   for (int pair = 0; pair < 2; ++pair) {
     if (pair && (g_cta2_mode == 1 || M <= 128)) continue;
     // the heuristic pairs only large, long-K plain GEMMs with N % 256 == 0 and the larger 3x3 convolutions
@@ -475,41 +575,52 @@ static void pick_tile(int M, int N, int num_kb, bool geglu, bool conv, int max_s
       if (g_force_bn && bn != g_force_bn && (N % g_force_bn == 0) && !geglu) continue;
       if (pair && bn < 128) continue;                    // per-CTA half of B must stay a whole number of KiB
       if (pair && g_cta2_mode == 0 && !conv && bn != 256) continue;
-      const int rows = pair ? 256 : 128;
-      const int tiles = ((M + rows - 1) / rows) * (N / bn);
-      const int units = pair ? sms / 2 : sms;
-      const float mma = 4.0f * bn;
-      const float l2 = 4.0f * (pair ? 128.0f + 0.5f * bn : 128.0f + bn);
-      const float per_kb = mma > l2 ? mma : l2;
-      for (int sp = 1; sp <= (pair ? 1 : max_splits); ++sp) {
-        if (sp > 1 && (num_kb / sp < (g_splitk_mode == 2 ? 4 : 16) || (long long)sp * M * N * 4 > ws_bytes)) break;
-        if (sp > 1 && tiles * 2 > units && g_splitk_mode != 2) break;        // only when the tile grid leaves >= half the SMs idle
-        if (g_splitk_mode == 2 && max_splits > 1 && sp == 1 && num_kb >= 8) continue;      // test hook: force a split
-        const int waves = (tiles * sp + units - 1) / units;
-        const int kb_cta = (num_kb + sp - 1) / sp;
-        float t = (float)waves * (per_kb * kb_cta + 3000.0f);
-        if (sp > 1) t += 12000.0f + (float)sp * M * N * 4.0f / (sms * 40.0f);     // slab round trip + reduce launch
-        const int ctas = (pair ? 2 : 1) * (tiles * sp < units ? tiles * sp : units);
-        t *= 1.0f + 0.10f * (1.0f - (float)ctas / (float)sms);     // idle SMs: prefer the finer decomposition
-        if (t < best) { best = t; best_bn = bn; best_pair = pair; best_s = sp; best_res = 0; }
-      }
-      // B-resident: one n-tile per CTA, weights loaded once per CTA, only A streams (plain GEMMs, single CTAs)
-      const int tiles_n = N / bn, tiles_m = (M + 127) / 128;
-      if (!pair && !conv && g_bres_mode != 1 && tiles_n <= sms && bres_stages(bn, num_kb) > 0) {
-        const int per_n = sms / tiles_n;
-        if (tiles_m >= 2 * per_n || g_bres_mode == 2) {
-          const int waves = (tiles_m + per_n - 1) / per_n;
-          const float l2a = 4.0f * 128.0f;
-          float t = (float)waves * ((mma > l2a ? mma : l2a) * num_kb + 3000.0f) + 4.0f * bn * num_kb;
-          const int ctas = per_n * tiles_n;
-          t *= 1.0f + 0.10f * (1.0f - (float)ctas / (float)sms);
-          if (g_bres_mode == 2) t = -1.0f / (float)bn;            // test hook: force (widest legal tile)
-          if (t < best) { best = t; best_bn = bn; best_pair = 0; best_s = 1; best_res = 1; }
+      for (int pp = 0; pp < 2; ++pp) {
+        // ping-pong holds 128 x BN fp32 accumulators per warpgroup in 168 registers: BN <= 128 (GEGLU: 128-row halves of
+        // the 256 tile); 128 x 160 spills
+        if (pp && (g_pp_mode == 1 || (!geglu && bn > 128))) continue;
+        if (pp && g_pp_mode == 0 && !pingpong_pays(M, bn, geglu, conv)) continue;
+        const int kbn = (pp && geglu) ? 128 : bn;        // width of one work item
+        // ping-pong where it measured ahead (heuristic) or wherever legal (test hook): preferred over every cooperative tile
+        const float force = pp ? 1e-3f : 1.0f;
+        const int rows = pair ? 256 : 128;
+        const int tiles = ((M + rows - 1) / rows) * (N / kbn);
+        const int units = pair ? sms / 2 : sms;
+        const float mma = 4.0f * kbn;
+        const float l2 = 4.0f * (pair ? 128.0f + 0.5f * kbn : 128.0f + kbn);
+        const float per_kb = mma > l2 ? mma : l2;
+        for (int sp = 1; sp <= (pair ? 1 : max_splits); ++sp) {
+          if (sp > 1 && (num_kb / sp < (g_splitk_mode == 2 ? 4 : 16) || (long long)sp * M * N * 4 > ws_bytes)) break;
+          if (sp > 1 && tiles * 2 > units && g_splitk_mode != 2) break;        // only when the tile grid leaves >= half the SMs idle
+          if (g_splitk_mode == 2 && max_splits > 1 && sp == 1 && num_kb >= 8) continue;      // test hook: force a split
+          const int waves = (tiles * sp + units - 1) / units;
+          const int kb_cta = (num_kb + sp - 1) / sp;
+          float t = (float)waves * (per_kb * kb_cta + 3000.0f);
+          if (sp > 1) t += 12000.0f + (float)sp * M * N * 4.0f / (sms * 40.0f);     // slab round trip + reduce launch
+          const int ctas = (pair ? 2 : 1) * (tiles * sp < units ? tiles * sp : units);
+          t *= 1.0f + 0.10f * (1.0f - (float)ctas / (float)sms);     // idle SMs: prefer the finer decomposition
+          t *= force;
+          if (t < best) { best = t; best_bn = bn; best_pair = pair; best_s = sp; best_res = 0; best_pp = pp; }
+        }
+        // B-resident: one n-tile per CTA, weights loaded once per CTA, only A streams (plain GEMMs, single CTAs)
+        const int tiles_n = N / kbn, tiles_m = (M + 127) / 128;
+        if (!pair && !conv && g_bres_mode != 1 && tiles_n <= sms && bres_stages(kbn, num_kb) > 0) {
+          const int per_n = sms / tiles_n;
+          if (tiles_m >= 2 * per_n || g_bres_mode == 2) {
+            const int waves = (tiles_m + per_n - 1) / per_n;
+            const float l2a = 4.0f * 128.0f;
+            float t = (float)waves * ((mma > l2a ? mma : l2a) * num_kb + 3000.0f) + 4.0f * kbn * num_kb;
+            const int ctas = per_n * tiles_n;
+            t *= 1.0f + 0.10f * (1.0f - (float)ctas / (float)sms);
+            if (g_bres_mode == 2) t = -1.0f / (float)bn / force;   // test hook: force (widest legal tile)
+            else t *= force;
+            if (t < best) { best = t; best_bn = bn; best_pair = 0; best_s = 1; best_res = 1; best_pp = pp; }
+          }
         }
       }
     }
   }
-  *bn_out = best_bn; *cta2_out = best_pair; *splits_out = best_s; *bres_out = best_res;
+  *bn_out = best_bn; *cta2_out = best_pair; *splits_out = best_s; *bres_out = best_res; *pp_out = best_pp;
 }
 
 }  // namespace glg
@@ -519,10 +630,17 @@ using namespace glg;
 extern "C" void glg_debug_force_bn(int bn) { glg::g_force_bn = bn; }
 // test hook (host only, no CUDA work): what the tile picker chooses for a problem; out[3] = {BN, paired CTAs, K splits}
 extern "C" void glg_debug_pick_tile(int M, int N, int K, int geglu, int conv, int can_split, long long ws_bytes, int* out) {
-  int bres = 0;
-  glg::pick_tile(M, N, (conv ? 9 : 1) * (K / 64), geglu != 0, conv != 0, can_split ? 8 : 1, ws_bytes, &out[0], &out[1], &out[2], &bres);
+  int bres = 0, pp = 0;
+  glg::pick_tile(M, N, (conv ? 9 : 1) * (K / 64), geglu != 0, conv != 0, can_split ? 8 : 1, ws_bytes, &out[0], &out[1], &out[2], &bres, &pp);
   out[1] |= bres << 8;           // bit 8 of the "paired" word: B-resident
 }
+// test hook (host only): 1 when the tile picker runs the problem on the ping-pong schedule
+extern "C" int glg_debug_pick_pingpong(int M, int N, int K, int geglu, int conv, int can_split, long long ws_bytes) {
+  int bn, pair, sp, bres, pp = 0;
+  glg::pick_tile(M, N, (conv ? 9 : 1) * (K / 64), geglu != 0, conv != 0, can_split ? 8 : 1, ws_bytes, &bn, &pair, &sp, &bres, &pp);
+  return pp;
+}
+extern "C" void glg_debug_gemm_pp(int mode) { glg::g_pp_mode = mode; }
 extern "C" void glg_debug_gemm_bres(int mode) { glg::g_bres_mode = mode; }
 extern "C" void glg_debug_gemm_cta2(int mode) { glg::g_cta2_mode = mode; }
 extern "C" void glg_debug_splitk(int mode) { glg::g_splitk_mode = mode; }
@@ -535,12 +653,13 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
   if (((uintptr_t)a->A | (uintptr_t)a->W | (uintptr_t)a->out | (uintptr_t)a->residual) & 15) return set_error("glg_gemm: pointers must be 16-byte aligned");
   if (a->rowbias && ((a->ld_rowbias % 4) || a->rows_per_batch <= 0)) return set_error("glg_gemm: bad rowbias args");
   if (a->geglu && (a->N % 256 || !a->bias || a->out_fp32)) return set_error("glg_gemm: geglu needs N % 256 == 0, a bias and bf16 output");
-  int bn = 0, cta2 = 0, splits = 1, bres = 0;
+  int bn = 0, cta2 = 0, splits = 1, bres = 0, pp = 0;
   const bool can_split = a->splitk_ws && g_splitk_mode != 1 && !a->geglu && !a->ln_stats && !a->stats_out && !a->out_fp32 &&
                          !((uintptr_t)a->splitk_ws & 15);
   pick_tile(a->M, a->N, (a->conv_mode ? 9 : 1) * (a->K / 64), a->geglu != 0, a->conv_mode != 0, can_split ? 8 : 1,
-            a->splitk_ws_bytes, &bn, &cta2, &splits, &bres);
+            a->splitk_ws_bytes, &bn, &cta2, &splits, &bres, &pp);
   if (!bn) return set_error("glg_gemm: N must be a multiple of 64");
+  const int kbn = (pp && a->geglu) ? 128 : bn;                     // width of one work item (ping-pong GEGLU: half a packed tile)
   GemmKParams p;
   memset(&p, 0, sizeof(p));
   const int rows_per_tile = cta2 ? 256 : 128;
@@ -548,7 +667,7 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
   p.kb_per_tap = a->K / 64;
   p.num_kb = a->conv_mode ? 9 * p.kb_per_tap : p.kb_per_tap;
   p.tiles_m = (a->M + rows_per_tile - 1) / rows_per_tile;
-  p.tiles_n = a->N / bn;
+  p.tiles_n = a->N / kbn;
   p.conv = a->conv_mode;
   p.out = a->out; p.ldc = a->ldc; p.out_fp32 = a->out_fp32;
   p.bias = a->bias; p.rowbias = a->rowbias; p.ld_rowbias = a->ld_rowbias; p.rows_per_batch = a->rows_per_batch > 0 ? a->rows_per_batch : 1;
@@ -573,8 +692,8 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
   p.splits = splits;
   p.ws = splits > 1 ? reinterpret_cast<float*>(a->splitk_ws) : nullptr;
   p.b_res = bres;
-  const long long stage_bytes = bres ? 16384 : 128 * 128 + bn * 128;
-  const long long fixed = bres ? (long long)p.num_kb * bn * 128 : 0;
+  const long long stage_bytes = bres ? 16384 : 128 * 128 + kbn * 128;
+  const long long fixed = bres ? (long long)p.num_kb * kbn * 128 : 0;
   long long stages = (kTileMax - fixed) / stage_bytes;
   const int cap = bres ? 12 : 8;
   p.stages = (int)(stages > cap ? cap : stages);
@@ -583,7 +702,8 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
   if (a->stats_out) p.stats_stride = a->stats_slot_stride > 0 ? a->stats_slot_stride : a->M;
   if (a->ln_stats) p.ln_stride = a->ln_slot_stride > 0 ? a->ln_slot_stride : a->M;
 
-  const uint32_t brows = (uint32_t)(cta2 ? bn / 2 : bn);           // a pair: each CTA multicasts half of the B tile
+  // a pair: each CTA multicasts half of the B tile; ping-pong GEGLU: x and gate rows are two boxes
+  const uint32_t brows = (uint32_t)(cta2 || (pp && a->geglu) ? kbn / 2 : kbn);
   CUtensorMap ta, tb;
   if (a->conv_mode) {
     const int H = a->H, W = a->Wd, B = a->Bn;
@@ -619,20 +739,33 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
     if (get_tmap_bf16(&tb, a->W, 2, wd, ws, wb)) return -1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (cta2) {
-    if (a->geglu) return launch_gemm<256, true, true>(ta, tb, p, smem, st);
+  if (pp) {
+    if (cta2) {
+      if (a->geglu) return launch_gemm<128, true, true, true>(ta, tb, p, smem, st);
+      switch (bn) {
+        case 128: return launch_gemm<128, false, true, true>(ta, tb, p, smem, st);
+      }
+    } else {
+      if (a->geglu) return launch_gemm<128, true, false, true>(ta, tb, p, smem, st);
+      switch (bn) {
+        case 128: return launch_gemm<128, false, false, true>(ta, tb, p, smem, st);
+        case 64:  return launch_gemm<64, false, false, true>(ta, tb, p, smem, st);
+      }
+    }
+  } else if (cta2) {
+    if (a->geglu) return launch_gemm<256, true, true, false>(ta, tb, p, smem, st);
     switch (bn) {
-      case 256: return launch_gemm<256, false, true>(ta, tb, p, smem, st);
-      case 160: return launch_gemm<160, false, true>(ta, tb, p, smem, st);
-      case 128: return launch_gemm<128, false, true>(ta, tb, p, smem, st);
+      case 256: return launch_gemm<256, false, true, false>(ta, tb, p, smem, st);
+      case 160: return launch_gemm<160, false, true, false>(ta, tb, p, smem, st);
+      case 128: return launch_gemm<128, false, true, false>(ta, tb, p, smem, st);
     }
   } else {
-    if (a->geglu) return launch_gemm<256, true, false>(ta, tb, p, smem, st);
+    if (a->geglu) return launch_gemm<256, true, false, false>(ta, tb, p, smem, st);
     switch (bn) {
-      case 256: return launch_gemm<256, false, false>(ta, tb, p, smem, st);
-      case 160: return launch_gemm<160, false, false>(ta, tb, p, smem, st);
-      case 128: return launch_gemm<128, false, false>(ta, tb, p, smem, st);
-      case 64:  return launch_gemm<64, false, false>(ta, tb, p, smem, st);
+      case 256: return launch_gemm<256, false, false, false>(ta, tb, p, smem, st);
+      case 160: return launch_gemm<160, false, false, false>(ta, tb, p, smem, st);
+      case 128: return launch_gemm<128, false, false, false>(ta, tb, p, smem, st);
+      case 64:  return launch_gemm<64, false, false, false>(ta, tb, p, smem, st);
     }
   }
   return set_error("glg_gemm: internal: bad tile");
