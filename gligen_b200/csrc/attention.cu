@@ -49,13 +49,19 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], uint32_t a0, uint3
       : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
+// not volatile: a pure function, so the scheduler may interleave the MUFU ops with each other and with the FMAs around them
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// exp2 of score pair j (0..7) of a 64-key tile: the last `poly` pairs of every 8 on the FMA pipe, the rest on the MUFU
-__device__ __forceinline__ float exp2_share(float x, int j, int poly) { return j >= 8 - poly ? ex2_poly3(x) : fast_exp2(x); }
+// exp2 of score pair j (0..7) of a 64-key tile.  POLY: the last `poly` pairs of every 8 on the FMA pipe, the rest on the
+// MUFU.  !POLY (the production instantiations): every exponential on the MUFU, with no per-pair compare and branch.
+template <bool POLY>
+__device__ __forceinline__ float exp2_share(float x, int j, int poly) {
+  if constexpr (POLY) return j >= 8 - poly ? ex2_poly3(x) : fast_exp2(x);
+  else return fast_exp2(x);
+}
 
 template <int DPAD>
 struct AttnCfg {
@@ -81,7 +87,7 @@ __device__ __forceinline__ void load_tile(uint32_t smem_tile, const bf16* g, lon
   }
 }
 
-template <int DPAD, bool SHORT>
+template <int DPAD, bool SHORT, bool POLY>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   // SHORT (Lk <= 128, the 77-token text context of cross attention): K and V (<= 2 tiles) are loaded ONCE and the
   // CTA walks QT = 4 consecutive 64-row query tiles with a double-buffered Q, instead of one CTA (and one K/V
@@ -201,10 +207,10 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
     uint32_t pa[8][2];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float p0 = exp2_share(fmaf(s[j][0], p.scale_log2, -ms0), j, p.poly);
-      const float p1 = exp2_share(fmaf(s[j][1], p.scale_log2, -ms0), j, p.poly);
-      const float p2 = exp2_share(fmaf(s[j][2], p.scale_log2, -ms1), j, p.poly);
-      const float p3 = exp2_share(fmaf(s[j][3], p.scale_log2, -ms1), j, p.poly);
+      const float p0 = exp2_share<POLY>(fmaf(s[j][0], p.scale_log2, -ms0), j, p.poly);
+      const float p1 = exp2_share<POLY>(fmaf(s[j][1], p.scale_log2, -ms0), j, p.poly);
+      const float p2 = exp2_share<POLY>(fmaf(s[j][2], p.scale_log2, -ms1), j, p.poly);
+      const float p3 = exp2_share<POLY>(fmaf(s[j][3], p.scale_log2, -ms1), j, p.poly);
       // the row sum uses the bf16-rounded probabilities that actually enter the PV product
       const uint32_t u01 = pack_bf16x2(p0, p1), u23 = pack_bf16x2(p2, p3);
       const float2 f01 = unpack_bf16x2(u01), f23 = unpack_bf16x2(u23);
@@ -288,11 +294,11 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnKParams p) {
   }
 }
 
-template <int DPAD, bool SHORT>
+template <int DPAD, bool SHORT, bool POLY>
 static int launch_attn2(const AttnKParams& p, int B, cudaStream_t st) {
   using Cfg = AttnCfg<DPAD>;
   static bool attr_set = false;
-  auto kern = attn_fwd_kernel<DPAD, SHORT>;
+  auto kern = attn_fwd_kernel<DPAD, SHORT, POLY>;
   constexpr int smem = (SHORT ? 6 : 5) * Cfg::TILE_ELEMS * 2;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -312,7 +318,13 @@ static int launch_attn2(const AttnKParams& p, int B, cudaStream_t st) {
 // in registers, O += P V with wgmma taking P straight from registers and V as a transposed (MN-major) operand.
 // Every tile is one 5-D TMA box {8 elements, rows, d/8 chunks, head, batch} that lands as [chunk][row][8 elements]: the
 // non-swizzled core-matrix layout wgmma reads, with the zero padding of d up to DPAD and of ragged rows done by the TMA.
-int g_attn_poly = 0;          // test hook (glg_debug_attn_poly_share): FMA-pipe share of the long-key kernels' exponentials
+// Each warpgroup runs its tiles strictly in order (QK^T, wait, softmax, PV, wait); the overlap comes from the other
+// warpgroup and the second resident CTA.  A software-pipelined loop (QK^T of tile j + 1 and PV of tile j in flight
+// together) and a ping-pong of the two warpgroups over named barriers were measured and are not ahead (DESIGN §5).
+// Registers per thread of the production (POLY = false) instantiations, 0 spill bytes in all: DPAD 16 / 32 / 48 / 64 /
+// 80: 66 / 74 / 82 / 93 / 112 -> 2 CTAs / SM (4 consumer warpgroups); DPAD 96 / 112 / 128 / 144 / 160: 132 / 140 / 135 /
+// 130 / 142 -> 1 CTA / SM.
+int g_attn_poly = 0;         // test hook (glg_debug_attn_poly_share): FMA-pipe share of the long-key kernels' exponentials
 
 template <int DPAD>
 struct HAttnCfg {
@@ -342,8 +354,9 @@ __device__ __forceinline__ uint64_t gmma_desc_interleave(uint32_t smem_addr, uin
   return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
 
-template <int DPAD>
-__global__ void __launch_bounds__(288, 1)
+// At most 112 registers up to DPAD 80, so that 2 CTAs (2 x 9 warps x 112 x 32) share an SM's 64K registers
+template <int DPAD, bool POLY>
+__global__ void __launch_bounds__(288) __maxnreg__(DPAD <= 80 ? 112 : 224)
 attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                   const __grid_constant__ CUtensorMap tmV, const HAttnParams p) {
   using Cfg = HAttnCfg<DPAD>;
@@ -437,20 +450,24 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     uint32_t pa[8][2];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const uint32_t u01 = pack_bf16x2(exp2_share(fmaf(sc[4 * j], p.scale_log2, -ms0), j, p.poly),
-                                       exp2_share(fmaf(sc[4 * j + 1], p.scale_log2, -ms0), j, p.poly));
-      const uint32_t u23 = pack_bf16x2(exp2_share(fmaf(sc[4 * j + 2], p.scale_log2, -ms1), j, p.poly),
-                                       exp2_share(fmaf(sc[4 * j + 3], p.scale_log2, -ms1), j, p.poly));
+      const uint32_t u01 = pack_bf16x2(exp2_share<POLY>(fmaf(sc[4 * j], p.scale_log2, -ms0), j, p.poly),
+                                       exp2_share<POLY>(fmaf(sc[4 * j + 1], p.scale_log2, -ms0), j, p.poly));
+      const uint32_t u23 = pack_bf16x2(exp2_share<POLY>(fmaf(sc[4 * j + 2], p.scale_log2, -ms1), j, p.poly),
+                                       exp2_share<POLY>(fmaf(sc[4 * j + 3], p.scale_log2, -ms1), j, p.poly));
       const float2 f01 = unpack_bf16x2(u01), f23 = unpack_bf16x2(u23);     // row sums of what enters P.V
       rs0 += f01.x + f01.y; rs1 += f23.x + f23.y;
       pa[j][0] = u01; pa[j][1] = u23;
     }
     l_run[0] = l_run[0] * corr0 + rs0;
     l_run[1] = l_run[1] * corr1 + rs1;
+    // Where no row of the warp moved its max, every corr is exactly 1 and the multiplies are skipped (x * 1.0f == x bit
+    // for bit).  The vote is warp-uniform, so the warp stays converged for the wgmma below.
+    if (!__all_sync(0xffffffffu, corr0 == 1.f && corr1 == 1.f)) {
 #pragma unroll
-    for (int j = 0; j < DT; ++j) {
-      o_acc[4 * j] *= corr0; o_acc[4 * j + 1] *= corr0;
-      o_acc[4 * j + 2] *= corr1; o_acc[4 * j + 3] *= corr1;
+      for (int j = 0; j < DT; ++j) {
+        o_acc[4 * j] *= corr0; o_acc[4 * j + 1] *= corr0;
+        o_acc[4 * j + 2] *= corr1; o_acc[4 * j + 3] *= corr1;
+      }
     }
     // ---- O += P V: V [chunk][64 keys][8] is the MN-major B operand (8-key groups 128 B apart, d chunks 1024 B apart)
     const uint64_t dv = gmma_desc_interleave(sV(s), 128u, 64u * 16u);
@@ -491,11 +508,11 @@ static int attn_tmap(CUtensorMap* m, const void* ptr, long long row, long long b
   return get_tmap_bf16_sw(m, ptr, 5, dims, str, box, 0);
 }
 
-template <int DPAD>
+template <int DPAD, bool POLY>
 static int launch_attn_wgmma(const GlgAttnArgs* a, cudaStream_t st) {
   using Cfg = HAttnCfg<DPAD>;
   static bool attr_set = false;
-  auto kern = attn_wgmma_kernel<DPAD>;
+  auto kern = attn_wgmma_kernel<DPAD, POLY>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (e != cudaSuccess) return set_error(std::string("cudaFuncSetAttribute(attn wgmma): ") + cudaGetErrorString(e));
@@ -517,6 +534,11 @@ static int launch_attn_wgmma(const GlgAttnArgs* a, cudaStream_t st) {
   return check_launch("attention (wgmma) launch");
 }
 
+template <int DPAD>
+static int launch_attn_wgmma(const GlgAttnArgs* a, cudaStream_t st) {
+  return g_attn_poly ? launch_attn_wgmma<DPAD, true>(a, st) : launch_attn_wgmma<DPAD, false>(a, st);
+}
+
 static int attention_wgmma(const GlgAttnArgs* a, cudaStream_t st) {
   switch ((a->d_head + 15) / 16 * 16) {
     case 16: return launch_attn_wgmma<16>(a, st);
@@ -535,7 +557,8 @@ static int attention_wgmma(const GlgAttnArgs* a, cudaStream_t st) {
 
 template <int DPAD>
 static int launch_attn(const AttnKParams& p, int B, bool short_keys, cudaStream_t st) {
-  return short_keys ? launch_attn2<DPAD, true>(p, B, st) : launch_attn2<DPAD, false>(p, B, st);
+  if (short_keys) return launch_attn2<DPAD, true, false>(p, B, st);      // p.poly is 0 for the short-key kernel
+  return p.poly ? launch_attn2<DPAD, false, true>(p, B, st) : launch_attn2<DPAD, false, false>(p, B, st);
 }
 
 int g_attn_mode = 0;          // test hook (glg_debug_attn_mode): 0 = auto (short-key mma.sync kernel for Lk <= 128, wgmma kernel above), 1 = the

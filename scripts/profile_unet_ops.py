@@ -7,7 +7,8 @@ set against each op's roofline lower bound, with the GEMM tile the picker chose.
 Writes OUT_DIR/profile.txt (one line per op, totals per kind and per category) and OUT_DIR/profile.json.  Op times come
 from bench.kernel_pass: every op replayed from its own CUDA graph and timed with CUDA events.  Bound = max(FLOP / 989 TFLOP/s,
 bytes / 3.35 TB/s): the H100 SXM data-sheet dense bf16 and HBM3 rates at 700 W, so on a power-capped card the bound is
-optimistic."""
+optimistic.  Attention rows also get the SFU bound (one ex2 per score at 16 / clk / SM, at the SM clock nvidia-smi reports
+after the pass), which is what limits small head dims, and are split by op (attn1 / fuser / attn2) and UNet level."""
 from __future__ import annotations
 
 import argparse
@@ -28,7 +29,13 @@ from gligen_b200 import synth  # noqa: E402
 from gligen_b200.spec import NAMED_CONFIGS, synthetic_state_dict  # noqa: E402
 
 PEAK_FLOPS, PEAK_BYTES = 989e12, 3.35e12
+SFU_PER_CLK = 16                                 # ex2 results / clk / SM
 LEVEL_OF_C = {320: 0, 640: 1, 1280: 2}
+
+
+def attention_category(name, heads, d):
+    op = "attn1" if ".attn1." in name else "fuser" if ".fuser." in name else "attn2" if ".attn2." in name else "attention"
+    return f"{op} L{LEVEL_OF_C.get(heads * d, '?')}"
 
 
 def card_info():
@@ -109,16 +116,24 @@ def main():
                     int(not geglu and kw.get("ln") is None and kw.get("stats_out") is None and out.dtype != torch.float32))
         return orig_gemm(x, w, out, **kw)
 
+    orig_attention = ops.attention
+
+    def attention(q, k, v, out, heads, d_head, causal=False):
+        cur["s"] = (q.shape[0], heads, d_head, q.shape[1], k.shape[1])
+        return orig_attention(q, k, v, out, heads, d_head, causal=causal)
+
     def note(kind, flops=0.0, nbytes=0.0):
         if ops.trace is not None:
             shapes.append(cur.pop("s", None))
         return orig_note(kind, flops, nbytes)
 
-    ops.gemm, ops._note = gemm, note
+    ops.gemm, ops.attention, ops._note = gemm, attention, note
     N = bt["boxes"].shape[1]
     agg, per_op = bench.kernel_pass(model, N, t["uc"].shape[1], a.batch, reps=a.reps)
-    ops.gemm, ops._note = orig_gemm, orig_note
+    ops.gemm, ops.attention, ops._note = orig_gemm, orig_attention, orig_note
     info = card_info()
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    sm_hz = float(info["clocks.sm"].split()[0]) * 1e6 if "clocks.sm" in info else 0.0
 
     lib = ops.lib
     import ctypes as C
@@ -142,6 +157,14 @@ def main():
             rec.update(M=M, N=Nn, K=K, taps=taps, geglu=geglu, bn=pick[0], pair=pick[1] & 255, resident=pick[1] >> 8, splits=pick[2], pp=pp)
             cat = category(name, kind, M, Nn, K, geglu)
             tile = f"{M:6d} {Nn:5d} {K:5d} {taps:3d} {pick[0]:3d} {pick[1] & 255:4d} {pick[1] >> 8:3d} {pick[2]:3d} {pp:2d}"
+        elif kind == "attention" and sh is not None:
+            B, heads, d, Lq, Lk = sh
+            sfu = B * heads * Lq * Lk / (SFU_PER_CLK * sms * sm_hz) * 1e3 if sm_hz else 0.0
+            if sfu > bound:
+                bound, by_what = sfu, "S"
+            rec.update(B=B, heads=heads, d=d, Lq=Lq, Lk=Lk, sfu_bound_ms=sfu, bound_ms=bound, bound_by=by_what)
+            cat = attention_category(name, heads, d)
+            tile = f"B{B} h{heads} d{d} {Lq}x{Lk}".ljust(47)
         else:
             cat = kind
             tile = " " * 47
