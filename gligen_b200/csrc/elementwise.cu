@@ -441,7 +441,9 @@ extern "C" int glg_conv_out(const void* x, int64_t ldx, const float* w, const fl
 }
 
 extern "C" int glg_softmax_rows(const float* s, int64_t lds, void* p, int64_t ldp, int64_t rows, int32_t cols, float scale, void* stream) {
-  if (cols <= 0 || cols % 4 || ldp % 2 || lds % 4) return set_error("glg_softmax_rows: cols % 4, lds % 4, ldp % 2 required");
+  // the kernel reads 4 scores as one float4 and writes 4 probabilities as one 8-byte store per thread and step
+  if (cols <= 0 || cols % 4 || ldp % 4 || lds % 4 || ((uintptr_t)s & 15) || ((uintptr_t)p & 7))
+    return set_error("glg_softmax_rows: cols % 4, lds % 4, ldp % 4, s 16-byte and p 8-byte aligned required");
   if (rows <= 0) return 0;
   launch_k(softmax_rows_kernel, dim3((unsigned)rows), dim3(256), 0, ST, 1, s, (long long)lds, (bf16*)p, (long long)ldp, cols, scale * 1.4426950408889634f);
   count_launch();

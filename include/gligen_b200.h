@@ -168,7 +168,8 @@ int glg_position_features(const float* feat, int64_t feat_batch_stride, const fl
                           const float* coords, const float* pos_mask, const float* null_pos, void* out, int64_t ldo,
                           int32_t B, int32_t N, int32_t F, int32_t ncoord, int32_t freqs, void* stream);
 /* Row softmax: p[r, c] = softmax_c(scale * s[r, c]) as bf16 (fp32 scores in, rows normalised before rounding).  The VAE
- * decoder's single-head attention over H*W tokens (model.py:178-202: torch.bmm + softmax + torch.bmm; head dim 512). */
+ * decoder's single-head attention over H*W tokens (model.py:178-202: torch.bmm + softmax + torch.bmm; head dim 512).
+ * cols, lds and ldp are multiples of 4; s is 16-byte and p 8-byte aligned. */
 int glg_softmax_rows(const float* s, int64_t lds, void* p, int64_t ldp, int64_t rows, int32_t cols, float scale, void* stream);
 /* fp32 -> bf16 cast of a contiguous buffer (context / weights staging). */
 int glg_cast_f32_bf16(const float* x, void* y, int64_t n, void* stream);

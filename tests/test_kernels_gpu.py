@@ -449,8 +449,13 @@ def test_small_ops(ops, ref):
     b = rnd(4, seed=2, dtype=torch.float32)
     out, out_r = torch.zeros(2, 4, 64, 64, device=dev), torch.zeros(2, 4, 64, 64, device=dev)
     ops.conv_out(x, w, b, out, 64, 64)
-    ref.conv_out(x, w, b, out_r, 64, 64)
-    assert_close(out, out_r, rel=2e-3, max_rel=5e-3, what="conv_out")   # torch reference conv runs in TF32
+    tf32 = torch.backends.cudnn.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False          # the checker must be fp32 (cuDNN convolutions default to TF32)
+    try:
+        ref.conv_out(x, w, b, out_r, 64, 64)
+    finally:
+        torch.backends.cudnn.allow_tf32 = tf32
+    assert_close(out, out_r, rel=1e-5, max_rel=1e-5, what="conv_out")   # fp32 against fp32: bf16 weights would be 1e-3
     # odd widths take the per-pixel kernels (the wide-latent variants need W % 4 / W % 8 == 0)
     x = rnd(2, 4, 10, 10, dtype=torch.float32)
     w = rnd(9, 4, 64, scale=0.2, seed=2, dtype=torch.float32)
@@ -464,8 +469,12 @@ def test_small_ops(ops, ref):
     b = rnd(4, seed=2, dtype=torch.float32)
     out, out_r = torch.zeros(2, 4, 10, 10, device=dev), torch.zeros(2, 4, 10, 10, device=dev)
     ops.conv_out(x, w, b, out, 10, 10)
-    ref.conv_out(x, w, b, out_r, 10, 10)
-    assert_close(out, out_r, rel=2e-3, max_rel=5e-3, what="conv_out 10x10")
+    torch.backends.cudnn.allow_tf32 = False
+    try:
+        ref.conv_out(x, w, b, out_r, 10, 10)
+    finally:
+        torch.backends.cudnn.allow_tf32 = tf32
+    assert_close(out, out_r, rel=1e-5, max_rel=1e-5, what="conv_out 10x10")
     # upsample / im2col
     x = rnd(2, 256, 640)
     y, y_r = torch.zeros(2, 1024, 640, device=dev, dtype=torch.bfloat16), torch.zeros(2, 1024, 640, device=dev, dtype=torch.bfloat16)
