@@ -103,7 +103,7 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// ------------------------------------------------------------------ TMA (tiled tensor maps)
+// ------------------------------------------------------------------ TMA (tiled and im2col tensor maps)
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }
@@ -113,10 +113,13 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, uint
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
+// im2col mode over (C, W, H, B): the map's pixels-per-column pixels, walked through its bounding box from position (w, h, n) in
+// (n, h, w) order, each read at (w + dw, h + dh)
+__device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst, const void* tmap, uint32_t bar, int c, int w, int h, int n,
+                                                   uint16_t dw, uint16_t dh) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(dw), "h"(dh)
       : "memory");
 }
 

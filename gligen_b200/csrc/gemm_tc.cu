@@ -30,11 +30,11 @@
 // A stages (the K = 320 / 640 projections), every CTA keeps ONE n-tile for its lifetime, loads that weight tile once and
 // streams only A tiles.
 //
-// conv_mode: the A operand is gathered by a 4-D tiled tensor map over the NHWC activation
-// (C, W, H, B); for tap (dy,dx) the box origin is shifted by (dx-1, dy-1) and TMA's out-of-bounds
-// zero fill implements the padding, so a 3x3 convolution is 9*Cin/64 K-steps of the same pipeline
-// with no im2col buffer.  A 128-row block is 128/W image rows (or 128/(H*W) whole images, or a 128-pixel segment of one
-// row when W > 128).
+// conv_mode: the A operand is gathered by an im2col-mode TMA map over the NHWC activation (C, W, H, B): a load of tap
+// (dy, dx) fills the 128 rows of an A stage with that tap's input pixel for 128 consecutive output pixels in (b, y, x)
+// order, across row and image boundaries, and TMA's out-of-bounds zero fill implements the padding.  A 3x3 convolution is
+// 9*Cin/64 K-steps of the same pipeline with no im2col buffer, and its 128-row blocks are those of a plain GEMM over the
+// B*H*W output pixels, at any H and W.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -367,11 +367,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int it = 0; get_work(it, tile, split, m_blk, n_blk); ++it) {
         const int kb_lo = (split * p.num_kb) / p.splits, kb_n = ((split + 1) * p.num_kb) / p.splits - kb_lo;
         const int row0 = m_blk * ROWS_PER_TILE + (int)rank * 128;
-        int b0 = 0, y0 = 0, x0 = 0;
+        int b0 = 0, y0 = 0, x0 = 0;                    // conv: the tile's first output pixel
         if (p.conv) {
           b0 = row0 / p.HW;
           y0 = (row0 - b0 * p.HW) / p.Wd;
-          x0 = row0 - b0 * p.HW - y0 * p.Wd;          // non-zero only for images wider than a tile (W > 128: part of one row)
+          x0 = row0 - b0 * p.HW - y0 * p.Wd;
         }
         // K steps are visited in a per-tile rotated order: tiles running at the same time would otherwise request
         // the very same weight (and activation) lines from L2 in lockstep; the rotation spreads them over slices.
@@ -388,8 +388,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (p.conv) {
               const int tap = kb / p.kb_per_tap;
               const int cb = kb - tap * p.kb_per_tap;
-              const int dy = tap / 3 - 1, dx = tap - (tap / 3) * 3 - 1;
-              tma_load_4d(a_dst, &tmA, full_bar(stage), cb * 64, x0 + dx, y0 + dy, b0);
+              const int dy = tap / 3, dx = tap - (tap / 3) * 3;
+              // bounding-box start (x0 - 1, y0 - 1): tap (0, 0) of the first output pixel
+              tma_load_im2col_4d(a_dst, &tmA, full_bar(stage), cb * 64, x0 - 1, y0 - 1, b0, (uint16_t)dx, (uint16_t)dy);
               ca = cb * 64; cb_off = tap * p.N;
             } else {
               tma_load_2d(a_dst, &tmA, full_bar(stage), kb * 64, row0);
@@ -708,22 +709,11 @@ extern "C" int glg_gemm(const GlgGemmArgs* a, void* stream) {
   if (a->conv_mode) {
     const int H = a->H, W = a->Wd, B = a->Bn;
     if (H <= 0 || W <= 0 || B <= 0 || (long long)B * H * W != a->M) return set_error("glg_gemm: conv dims do not match M");
-    if ((W <= 128 && (128 % W)) || (W > 128 && (W % 128))) return set_error("glg_gemm: conv width must divide 128 or be a multiple of it");
     const int HW = H * W;
-    uint32_t box[4];
-    if (W > 128) {                 // a 128-pixel tile is a segment of one image row (VAE decoder: 256 / 512 wide)
-      box[0] = 64; box[1] = 128; box[2] = 1; box[3] = 1;
-    } else if (HW >= 128) {
-      if (HW % 128) return set_error("glg_gemm: conv H*W must be a multiple of 128 (or divide it)");
-      box[0] = 64; box[1] = W; box[2] = 128 / W; box[3] = 1;
-    } else {
-      if (128 % HW) return set_error("glg_gemm: conv H*W must divide 128");
-      box[0] = 64; box[1] = W; box[2] = H; box[3] = 128 / HW;
-    }
     p.HW = HW; p.Wd = W;
     const uint64_t dims[4] = {(uint64_t)a->K, (uint64_t)W, (uint64_t)H, (uint64_t)B};
     const uint64_t str[3] = {(uint64_t)a->lda * 2, (uint64_t)a->lda * 2 * W, (uint64_t)a->lda * 2 * HW};
-    if (get_tmap_bf16(&ta, a->A, 4, dims, str, box)) return -1;
+    if (get_tmap_bf16_im2col3x3(&ta, a->A, dims, str, 64, 128)) return -1;
     const uint64_t wd[2] = {(uint64_t)a->K, (uint64_t)a->N * 9};
     const uint64_t ws[1] = {(uint64_t)a->K * 2};
     const uint32_t wb[2] = {64, brows};

@@ -17,6 +17,9 @@ int check_launch(const char* what);
 int get_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box);
 // swizzle_bytes: 0 (none), 64 or 128; rank 1..5
 int get_tmap_bf16_sw(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box, int swizzle_bytes);
+// bf16 im2col map (128B swizzle, zero OOB fill) for the 3x3 / pad 1 / stride 1 convolution over NHWC dims (C, W, H, B):
+// `channels` x `pixels` per load, see tma_host.cu
+int get_tmap_bf16_im2col3x3(CUtensorMap* out, const void* ptr, const uint64_t* dims, const uint64_t* strides, uint32_t channels, uint32_t pixels);
 int num_sms();
 bool pdl_enabled();     // GLG_PDL env (default off)
 int pdl_mode();         // 0 off, 1 every launch, 2 only launches whose grid leaves SMs idle (fewer CTAs than SMs): their prologue

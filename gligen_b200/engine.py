@@ -55,7 +55,7 @@ class Engine(EngineBase):
         self.cfg = cfg
         self.blocks = block_schedule(cfg)
         self.W: Dict[str, torch.Tensor] = {}
-        self.plans: Dict[Tuple[int, int, int], Plan] = {}
+        self.plans: Dict[Tuple[int, ...], Plan] = {}
         self.scale = 1.0
         self.use_graphs = use_graphs and self.dev.type == "cuda"
         self.loaded = False
@@ -261,12 +261,10 @@ class Engine(EngineBase):
         self._plan_allocs.append(t)
         return t
 
-    def _sizes(self, Bt: int, N: int, nctx: int) -> Dict[str, int]:
-        cfg = self.cfg
-        G = N * self.n_streams
+    def _sizes(self, Bt: int, N: int, nctx: int, Hl: int, Wl: int) -> Dict[str, int]:
         s = dict(t0=0, sb=0, sc=0, sd=0, up=0, col=0, xs=0, qkv=0, ao=0, ffh=0, xstat=0, blk=0)
         for blk in self.blocks:
-            hw = (cfg.image_size // blk.ds) ** 2
+            hw = (Hl // blk.ds) * (Wl // blk.ds)
             for ly in blk.layers:
                 if ly.kind == "res":
                     s["t0"] = max(s["t0"], Bt * hw * ly.cin)
@@ -287,17 +285,17 @@ class Engine(EngineBase):
                     s["up"] = max(s["up"], Bt * hw * 4 * ly.cin)
         return s
 
-    def _build_plan(self, Bt: int, N: int, nctx: int) -> Plan:
+    def _build_plan(self, Bt: int, N: int, nctx: int, Hl: int, Wl: int) -> Plan:
+        """Plan for a [Bt, in_channels, Hl, Wl] latent."""
         cfg, ops, W = self.cfg, self.ops, self.W
         S = self.n_streams
         G = N * S
         P = Plan()
         self._plan_allocs = P.buffers = []
-        sz = self._sizes(Bt, N, nctx)
+        sz = self._sizes(Bt, N, nctx, Hl, Wl)
         B_ = {k: self._buf(v, torch.float32 if k == "xstat" else None) for k, v in sz.items()}
         B_["blk2"] = self._buf(sz["blk"])
         stats = self._zeros(gn_scratch_floats(Bt))   # GLG_GN_SCRATCH_FLOATS, barrier counters zeroed once
-        Himg = cfg.image_size
         f32 = torch.float32
 
         def view(name, *shape):
@@ -307,9 +305,9 @@ class Engine(EngineBase):
             return B_[name][:n].view(*shape)
 
         # ---- static inputs -------------------------------------------------------------------
-        P.inp["x"] = self._zeros(Bt, cfg.in_channels, Himg, Himg)
+        P.inp["x"] = self._zeros(Bt, cfg.in_channels, Hl, Wl)
         if cfg.inpaint_mode:
-            P.inp["extra"] = self._zeros(Bt, cfg.in_channels + 1, Himg, Himg)
+            P.inp["extra"] = self._zeros(Bt, cfg.in_channels + 1, Hl, Wl)
         P.inp["t"] = self._zeros(Bt, dtype=torch.int64)
         P.inp["context"] = self._zeros(Bt, nctx, cfg.context_dim)
         if cfg.spatial:
@@ -326,7 +324,7 @@ class Engine(EngineBase):
             for si in range(S):
                 P.inp[f"feat{si}"] = self._zeros(Bt, N, cfg.tok_in_dim)
                 P.inp[f"fmask{si}"] = self._zeros(Bt, N)
-        P.out = self._zeros(Bt, cfg.out_channels, Himg, Himg)
+        P.out = self._zeros(Bt, cfg.out_channels, Hl, Wl)
 
         # ---- grounding tokens (PositionNet) -> objs [S, Bt*N, D] -----------------------------
         D = cfg.tok_out_dim
@@ -376,7 +374,7 @@ class Engine(EngineBase):
         mid = [b for b in self.blocks if b.where == "mid"][0]
         cats = []
         for ob in out_blocks:
-            hw = (Himg // ob.ds) ** 2
+            hw = (Hl // ob.ds) * (Wl // ob.ds)
             ctot = ob.layers[0].cin
             cats.append(self._buf(Bt * hw * ctot).view(Bt, hw, ctot))
         dest: Dict[Tuple[str, int], torch.Tensor] = {}
@@ -390,13 +388,13 @@ class Engine(EngineBase):
             if i + 1 < len(out_blocks):
                 dest[("out", ob.index)] = cats[i + 1][:, :, : ob.out_ch]
             else:
-                dest[("out", ob.index)] = self._buf(Bt * Himg * Himg * ob.out_ch).view(Bt, Himg * Himg, ob.out_ch)
+                dest[("out", ob.index)] = self._buf(Bt * Hl * Wl * ob.out_ch).view(Bt, Hl * Wl, ob.out_ch)
 
         st_index = {p: i for i, p in enumerate(self.st_prefixes)}
 
         # ---- layer emitters --------------------------------------------------------------------
-        def emit_res(ly, x, out, H):
-            p, hw = ly.prefix, H * H
+        def emit_res(ly, x, out, H, Wd):
+            p, hw = ly.prefix, H * Wd
             a = view("t0", Bt, hw, ly.cin)
             h1 = view("sb", Bt, hw, ly.cout)
             a2 = view("sc", Bt, hw, ly.cout)
@@ -404,7 +402,7 @@ class Engine(EngineBase):
             rb = emb_all[:, off: off + ly.cout]
             P.add(f"{p}.gn1", lambda: ops.groupnorm(x, a, W[f"{p}.gn1.g"], W[f"{p}.gn1.b"], stats, 32, 1e-5, True))
             P.add(f"{p}.conv1", lambda: ops.gemm(a, W[f"{p}.conv1.w"], h1, bias=W[f"{p}.conv1.b"], rowbias=rb,
-                                                 rows_per_batch=hw, conv=(Bt, H, H)))
+                                                 rows_per_batch=hw, conv=(Bt, H, Wd)))
             P.add(f"{p}.gn2", lambda: ops.groupnorm(h1, a2, W[f"{p}.gn2.g"], W[f"{p}.gn2.b"], stats, 32, 1e-5, True))
             if ly.cin != ly.cout:
                 sk = view("sd", Bt, hw, ly.cout)
@@ -412,10 +410,10 @@ class Engine(EngineBase):
                 res = sk
             else:
                 res = x
-            P.add(f"{p}.conv2", lambda: ops.gemm(a2, W[f"{p}.conv2.w"], out, bias=W[f"{p}.conv2.b"], residual=res, conv=(Bt, H, H)))
+            P.add(f"{p}.conv2", lambda: ops.gemm(a2, W[f"{p}.conv2.w"], out, bias=W[f"{p}.conv2.b"], residual=res, conv=(Bt, H, Wd)))
 
-        def emit_st(ly, x_in, out, H):
-            p, T, C = ly.prefix, H * H, ly.cin
+        def emit_st(ly, x_in, out, H, Wd):
+            p, T, C = ly.prefix, H * Wd, ly.cin
             tb = f"{p}.transformer_blocks.0"
             heads, d = ly.heads, ly.d_head
             gi = st_index[p]
@@ -468,24 +466,23 @@ class Engine(EngineBase):
             P.add(f"{tb}.ff.2", lambda: ops.gemm(ffh, W[f"{tb}.ff.w2"], xs, bias=W[f"{tb}.ff.b2"], residual=xs))
             P.add(f"{p}.proj_out", lambda: ops.gemm(xs, W[f"{p}.proj_out.w"], out, bias=W[f"{p}.proj_out.b"], residual=x_in))
 
-        def emit_down(ly, x, out, H):
+        def emit_down(ly, x, out, H, Wd):
             p = ly.prefix
-            Ho = H // 2
-            col = view("col", Bt * Ho * Ho, 9 * ly.cin)
-            P.add(f"{p}.im2col", lambda: ops.im2col_s2(x, col, H, H))
+            col = view("col", Bt * (H // 2) * (Wd // 2), 9 * ly.cin)
+            P.add(f"{p}.im2col", lambda: ops.im2col_s2(x, col, H, Wd))
             P.add(f"{p}.conv", lambda: ops.gemm(col, W[f"{p}.w"], out, bias=W[f"{p}.b"]))
 
-        def emit_up(ly, x, out, H):
+        def emit_up(ly, x, out, H, Wd):
             p = ly.prefix
-            up = view("up", Bt, 4 * H * H, ly.cin)
-            P.add(f"{p}.upsample", lambda: ops.upsample2x(x, up, H, H))
-            P.add(f"{p}.conv", lambda: ops.gemm(up, W[f"{p}.w"], out, bias=W[f"{p}.b"], conv=(Bt, 2 * H, 2 * H)))
+            up = view("up", Bt, 4 * H * Wd, ly.cin)
+            P.add(f"{p}.upsample", lambda: ops.upsample2x(x, up, H, Wd))
+            P.add(f"{p}.conv", lambda: ops.gemm(up, W[f"{p}.w"], out, bias=W[f"{p}.b"], conv=(Bt, 2 * H, 2 * Wd)))
 
         # ---- walk the blocks ---------------------------------------------------------------------
         h = None
         oi = 0
         for blk in self.blocks:
-            H = Himg // blk.ds
+            H, Wd = Hl // blk.ds, Wl // blk.ds
             if blk.where == "out":
                 h = cats[oi]
                 oi += 1
@@ -493,35 +490,55 @@ class Engine(EngineBase):
             tmp_names = ["blk", "blk2"]
             for li, ly in enumerate(blk.layers):
                 last = li == len(blk.layers) - 1
-                o = final if last else view(tmp_names[li % 2], Bt, H * H, ly.cout)
+                o = final if last else view(tmp_names[li % 2], Bt, H * Wd, ly.cout)
                 if ly.kind == "conv_in":
                     extra = P.inp.get("extra") if ds_planes is None else ds_planes
                     P.add("conv_in", lambda o=o, extra=extra: ops.conv_in(P.inp["x"], extra, W["conv_in.w"], W["conv_in.b"], o))
                 elif ly.kind == "res":
-                    emit_res(ly, h, o, H)
+                    emit_res(ly, h, o, H, Wd)
                 elif ly.kind == "st":
-                    emit_st(ly, h, o, H)
+                    emit_st(ly, h, o, H, Wd)
                 elif ly.kind == "down":
-                    emit_down(ly, h, o, H)
+                    emit_down(ly, h, o, H, Wd)
                 elif ly.kind == "up":
-                    emit_up(ly, h, o, H)
+                    emit_up(ly, h, o, H, Wd)
                 h = o
         # ---- out: GN + SiLU + conv3x3 -> eps (NCHW fp32) ----------------------------------------
         mc = cfg.model_channels
-        fin = view("t0", Bt, Himg * Himg, mc)
+        fin = view("t0", Bt, Hl * Wl, mc)
         hl = h
         P.add("out.gn", lambda: ops.groupnorm(hl, fin, W["out.gn.g"], W["out.gn.b"], stats, 32, 1e-5, True))
-        P.add("out.conv", lambda: ops.conv_out(fin, W["out.w"], W["out.b"], P.out, Himg, Himg))
+        P.add("out.conv", lambda: ops.conv_out(fin, W["out.w"], W["out.b"], P.out, Hl, Wl))
         return P
 
     # ------------------------------------------------------------------------------------------
     # execution
     # ------------------------------------------------------------------------------------------
-    def _plan(self, Bt: int, N: int, nctx: int, slot: int = 0) -> Plan:
-        key = (Bt, N, nctx) if slot == 0 else (Bt, N, nctx, slot)       # one plan (and static-part cache) per batch chunk
+    def _plan(self, Bt: int, N: int, nctx: int, slot: int = 0, H: Optional[int] = None, W: Optional[int] = None) -> Plan:
+        """Plan for Bt rows of an H x W latent (default: cfg.image_size square)."""
+        H = self.cfg.image_size if H is None else H
+        W = self.cfg.image_size if W is None else W
+        self.check_latent_size(H, W)
+        # one plan (and static-part cache) per latent size and batch chunk; the square default size keeps the short key
+        size = () if H == W == self.cfg.image_size else (H, W)
+        key = (Bt, N, nctx) + size + ((slot,) if slot else ())
         if key not in self.plans:
-            self.plans[key] = self._build_plan(Bt, N, nctx)
+            self.plans[key] = self._build_plan(Bt, N, nctx, H, W)
         return self.plans[key]
+
+    def check_latent_size(self, H: int, W: int) -> None:
+        """Latent sides must survive every stride-2 downsample exactly (the reference fails on other sides at the skip
+        concatenation, openaimodel.py:461).  A grounding downsampler writes planes of one fixed size (hed_grounding_downsampler.py:
+        interpolate to 64 x 64) that conv_in concatenates, so those models run at their native latent size only - also after
+        restore_first_conv_from_SD, where the reference itself would run at other sizes (the plan keeps reading the planes
+        through zero weights)."""
+        f = max(blk.ds for blk in self.blocks)
+        if H <= 0 or W <= 0 or H % f or W % f:
+            raise ValueError(f"latent {H}x{W}: both sides must be positive multiples of {f} (one per stride-2 downsample)")
+        n = self.cfg.image_size
+        if self.cfg.ds_out_dim and (H, W) != (n, n):
+            raise ValueError(f"latent {H}x{W}: the grounding downsampler of {self.cfg.tokenizer} models writes {n}x{n} planes that "
+                             f"conv_in concatenates with the latent, so this model runs at {n}x{n} only (also with the SD first conv restored)")
 
     def _n_objs(self, grounding: Dict[str, torch.Tensor]) -> int:
         if self.cfg.spatial:
@@ -667,7 +684,7 @@ class Engine(EngineBase):
                                "of the last prepared one (GroundingNetInput.get_null_input asserts the same)")
         else:
             N = self._last_N
-        P = self._plan(B, N, context.shape[1], slot)
+        P = self._plan(B, N, context.shape[1], slot, *x.shape[2:])
         P.inp["x"].copy_(x)
         P.inp["t"].copy_(timesteps)
         if self.cfg.inpaint_mode:
@@ -702,7 +719,7 @@ class Engine(EngineBase):
         B = x.shape[0]
         N = self._n_objs(grounding)
         self._last_N = N
-        P = self._plan(2 * B, N, context.shape[1], slot)
+        P = self._plan(2 * B, N, context.shape[1], slot, *x.shape[2:])
         P.inp["x"][:B].copy_(x); P.inp["x"][B:].copy_(x)
         P.inp["t"][:B].copy_(timesteps); P.inp["t"][B:].copy_(timesteps)
         if self.cfg.inpaint_mode:

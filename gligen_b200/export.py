@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import ctypes as C
 import struct
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -51,12 +51,13 @@ def _registry(eng, P) -> List[Tuple[str, torch.Tensor, bool]]:
     return reg
 
 
-def export_plan(eng, rows: int, n_objs: int, n_ctx: int, path: str) -> Dict[str, int]:
-    """Write the plan for (rows, n_objs, n_ctx) - rows = 2B when cond + uncond run as one batch.  Returns counts.
+def export_plan(eng, rows: int, n_objs: int, n_ctx: int, path: str, H: Optional[int] = None, W: Optional[int] = None) -> Dict[str, int]:
+    """Write the plan for (rows, n_objs, n_ctx) at an H x W latent (default: the config's square size) - rows = 2B when cond +
+    uncond run as one batch.  The latent size is baked into the recorded calls and the sizes of "in:x" / "out".  Returns counts.
     Spatial-map models: n_objs = cfg.spatial_tokens, and the engine must have seen one grounded call (or `eng._n_objs(grounding)`)
     so that it knows the (C, H, W) of the conditioning map its static buffers are sized for; the named inputs are then
     "in:map", "in:gmask" and "in:extra_map"."""
-    P = eng._plan(rows, n_objs, n_ctx)
+    P = eng._plan(rows, n_objs, n_ctx, H=H, W=W)
     reg = _registry(eng, P)
     spans = []
     for bi, (name, t, _) in enumerate(reg):

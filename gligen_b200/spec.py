@@ -400,12 +400,14 @@ def synthetic_state_dict(cfg: UNetConfig, seed: int = 0) -> Dict[str, torch.Tens
     return sd
 
 
-def flops_per_forward(cfg: UNetConfig, G: int, fuser_on: bool = True) -> float:
-    """Algorithmic 2*MAC of one UNet forward for ONE sample (SURVEY 8d analytic generator)."""
+def flops_per_forward(cfg: UNetConfig, G: int, fuser_on: bool = True, latent: Optional[Tuple[int, int]] = None) -> float:
+    """Algorithmic 2*MAC of one UNet forward for ONE sample (SURVEY 8d analytic generator); latent = (H, W), default square
+    cfg.image_size."""
     ctx, ted = cfg.context_dim, cfg.time_embed_dim
+    Hl, Wl = latent or (cfg.image_size, cfg.image_size)
     total = 0.0
     for blk in block_schedule(cfg):
-        hw = (cfg.image_size // blk.ds) ** 2
+        hw = (Hl // blk.ds) * (Wl // blk.ds)
         for ly in blk.layers:
             if ly.kind == "conv_in":
                 total += 18.0 * hw * ly.cin * ly.cout
@@ -425,7 +427,7 @@ def flops_per_forward(cfg: UNetConfig, G: int, fuser_on: bool = True) -> float:
                 total += 18.0 * (hw // 4) * ly.cin * ly.cout
             elif ly.kind == "up":
                 total += 18.0 * (hw * 4) * ly.cin * ly.cout
-    total += 18.0 * cfg.image_size ** 2 * cfg.model_channels * cfg.out_channels
+    total += 18.0 * Hl * Wl * cfg.model_channels * cfg.out_channels
     total += 2.0 * (cfg.model_channels * ted + ted * ted)
     if cfg.spatial:
         return total          # the ConvNeXt tokenizer runs once per sample, not per forward

@@ -74,25 +74,27 @@ class _VAEEngineBase(EngineBase):
         self.ops.groupnorm(x, y, g, b, stats, 32, 1e-6, silu)
         return y
 
-    def _resblock(self, x, prefix, B, H, stats):
+    def _resblock(self, x, prefix, B, H, Wd, stats):
         ops, W = self.ops, self.W
         cout = W[f"{prefix}.conv1.b"].numel()
         h = self._gn(x, W[f"{prefix}.norm1.g"], W[f"{prefix}.norm1.b"], True, stats)
-        h1 = self._buf(B, H * H, cout)
-        ops.gemm(h, W[f"{prefix}.conv1.w"], h1, bias=W[f"{prefix}.conv1.b"], conv=(B, H, H))
+        h1 = self._buf(B, H * Wd, cout)
+        ops.gemm(h, W[f"{prefix}.conv1.w"], h1, bias=W[f"{prefix}.conv1.b"], conv=(B, H, Wd))
         h = self._gn(h1, W[f"{prefix}.norm2.g"], W[f"{prefix}.norm2.b"], True, stats)
         if f"{prefix}.nin.w" in W:
-            sk = self._buf(B, H * H, cout)
+            sk = self._buf(B, H * Wd, cout)
             ops.gemm(x, W[f"{prefix}.nin.w"], sk, bias=W[f"{prefix}.nin.b"])
         else:
             sk = x
-        out = self._buf(B, H * H, cout)
-        ops.gemm(h, W[f"{prefix}.conv2.w"], out, bias=W[f"{prefix}.conv2.b"], residual=sk, conv=(B, H, H))
+        out = self._buf(B, H * Wd, cout)
+        ops.gemm(h, W[f"{prefix}.conv2.w"], out, bias=W[f"{prefix}.conv2.b"], residual=sk, conv=(B, H, Wd))
         return out
 
-    def _attn(self, x, a, B, H, stats):
+    def _attn(self, x, a, B, H, Wd, stats):
+        """T = H * Wd tokens; the P.V GEMM has K = T, so T must be a multiple of 64.  The fp32 T x T score matrix is
+        materialised (1 GiB at T = 16384, a 1024 x 1024 image)."""
         ops, W = self.ops, self.W
-        T, C = H * H, x.shape[-1]
+        T, C = H * Wd, x.shape[-1]
         hn = self._gn(x, W[f"{a}.norm.g"], W[f"{a}.norm.b"], False, stats)
         q, k = self._buf(B, T, C), self._buf(B, T, C)
         ops.gemm(hn, W[f"{a}.q.w"], q, bias=W[f"{a}.q.b"])
@@ -147,30 +149,32 @@ class VAEDecoderEngine(_VAEEngineBase):
         assert self.loaded, "load_state_dict first"
         cfg, ops, W = self.cfg, self.ops, self.W
         B, _, H, Wd = z.shape
-        assert H == Wd, "square latents only"
+        if H <= 0 or Wd <= 0 or H % 8 or Wd % 8:
+            # the mid attention's P.V GEMM reduces over h*w tokens, which must be a multiple of 64
+            raise ValueError(f"latent {H}x{Wd}: both sides must be positive multiples of 8")
         z = z.to(device=self.dev, dtype=torch.float32).contiguous()
-        ones = torch.ones(B, 1, H, H, device=self.dev, dtype=torch.float32)
+        ones = torch.ones(B, 1, H, Wd, device=self.dev, dtype=torch.float32)
         stats = torch.zeros(gn_scratch_floats(B), device=self.dev, dtype=torch.float32)
         block_in = cfg.ch * cfg.ch_mult[-1]
-        h = self._buf(B, H * H, block_in)
+        h = self._buf(B, H * Wd, block_in)
         ops.conv_in(z, ones, W["conv_in.w"], W["conv_in.b"], h)
-        h = self._resblock(h, "decoder.mid.block_1", B, H, stats)
-        h = self._attn(h, "decoder.mid.attn_1", B, H, stats)
-        h = self._resblock(h, "decoder.mid.block_2", B, H, stats)
+        h = self._resblock(h, "decoder.mid.block_1", B, H, Wd, stats)
+        h = self._attn(h, "decoder.mid.attn_1", B, H, Wd, stats)
+        h = self._resblock(h, "decoder.mid.block_2", B, H, Wd, stats)
         for i_level in reversed(range(len(cfg.ch_mult))):
             for i_block in range(cfg.num_res_blocks + 1):
-                h = self._resblock(h, f"decoder.up.{i_level}.block.{i_block}", B, H, stats)
+                h = self._resblock(h, f"decoder.up.{i_level}.block.{i_block}", B, H, Wd, stats)
             if i_level != 0:
                 C = h.shape[-1]
-                up = self._buf(B, 4 * H * H, C)
-                ops.upsample2x(h, up, H, H)
-                H *= 2
-                h = self._buf(B, H * H, C)
+                up = self._buf(B, 4 * H * Wd, C)
+                ops.upsample2x(h, up, H, Wd)
+                H, Wd = 2 * H, 2 * Wd
+                h = self._buf(B, H * Wd, C)
                 p = f"decoder.up.{i_level}.upsample.conv"
-                ops.gemm(up, W[f"{p}.w"], h, bias=W[f"{p}.b"], conv=(B, H, H))
+                ops.gemm(up, W[f"{p}.w"], h, bias=W[f"{p}.b"], conv=(B, H, Wd))
         h = self._gn(h, W["norm_out.g"], W["norm_out.b"], True, stats)
-        img = torch.empty(B, cfg.out_ch, H, H, device=self.dev, dtype=torch.float32)
-        ops.conv_out(h, W["conv_out.w"], W["conv_out.b"], img, H, H)
+        img = torch.empty(B, cfg.out_ch, H, Wd, device=self.dev, dtype=torch.float32)
+        ops.conv_out(h, W["conv_out.w"], W["conv_out.b"], img, H, Wd)
         return img
 
 
@@ -206,33 +210,37 @@ class VAEEncoderEngine(_VAEEngineBase):
 
     @torch.no_grad()
     def encode_moments(self, x: torch.Tensor) -> torch.Tensor:
-        """x: fp32 image [B, in_channels, S, S] -> moments fp32 [B, 2 * embed_dim, S / 2^(levels-1), ...]."""
+        """x: fp32 image [B, in_channels, H, W] -> moments fp32 [B, 2 * embed_dim, H / 2^(levels-1), W / 2^(levels-1)]."""
         assert self.loaded, "load_state_dict first"
         cfg, ops, W = self.cfg, self.ops, self.W
         B, Cin, H, Wd = x.shape
         nlev = len(cfg.ch_mult)
-        assert H == Wd and Cin == cfg.in_channels and H % (1 << (nlev - 1)) == 0, "square images, side a multiple of 2^(levels-1)"
+        assert Cin == cfg.in_channels, (Cin, cfg.in_channels)
+        f = 1 << (nlev - 1)
+        if H <= 0 or Wd <= 0 or H % f or Wd % f:
+            # one factor 2 per stride-2 downsample.  On the GPU the mid attention's P.V GEMM also needs (H/f)*(W/f) to be a
+            # multiple of 64, which glg_gemm reports itself.
+            raise ValueError(f"image {H}x{Wd}: both sides must be positive multiples of {f}")
         x = x.to(device=self.dev, dtype=torch.float32).contiguous()
         stats = torch.zeros(gn_scratch_floats(B), device=self.dev, dtype=torch.float32)
-        h = self._buf(B, H * H, cfg.ch)
+        h = self._buf(B, H * Wd, cfg.ch)
         ops.conv_in(x, None, W["conv_in.w"], W["conv_in.b"], h)
         for i_level in range(nlev):
             for i_block in range(cfg.num_res_blocks):
-                h = self._resblock(h, f"encoder.down.{i_level}.block.{i_block}", B, H, stats)
+                h = self._resblock(h, f"encoder.down.{i_level}.block.{i_block}", B, H, Wd, stats)
             if i_level != nlev - 1:
                 p = f"encoder.down.{i_level}.downsample.conv"
                 C = h.shape[-1]
-                Ho = H // 2
-                col = self._buf(B * Ho * Ho, 9 * C)
-                ops.im2col_s2(h, col, H, H, pad_lo=0)
-                h = self._buf(B, Ho * Ho, C)
+                col = self._buf(B * (H // 2) * (Wd // 2), 9 * C)
+                ops.im2col_s2(h, col, H, Wd, pad_lo=0)
+                H, Wd = H // 2, Wd // 2
+                h = self._buf(B, H * Wd, C)
                 ops.gemm(col, W[p + ".w"], h, bias=W[p + ".b"])
                 del col
-                H = Ho
-        h = self._resblock(h, "encoder.mid.block_1", B, H, stats)
-        h = self._attn(h, "encoder.mid.attn_1", B, H, stats)
-        h = self._resblock(h, "encoder.mid.block_2", B, H, stats)
+        h = self._resblock(h, "encoder.mid.block_1", B, H, Wd, stats)
+        h = self._attn(h, "encoder.mid.attn_1", B, H, Wd, stats)
+        h = self._resblock(h, "encoder.mid.block_2", B, H, Wd, stats)
         h = self._gn(h, W["norm_out.g"], W["norm_out.b"], True, stats)
-        mom = torch.empty(B, 2 * cfg.embed_dim, H, H, device=self.dev, dtype=torch.float32)
-        ops.conv_out(h, W["conv_out.w"], W["conv_out.b"], mom, H, H)
+        mom = torch.empty(B, 2 * cfg.embed_dim, H, Wd, device=self.dev, dtype=torch.float32)
+        ops.conv_out(h, W["conv_out.w"], W["conv_out.b"], mom, H, Wd)
         return mom

@@ -49,7 +49,7 @@ void glg_reset_launch_count(void);
  *                           v = act(v);   v *= *gate;   v += residual[row][n];
  * geglu=1 (attention.py:42-44): W/bias rows are packed per 256-row tile as [128 x-rows | 128 gate-rows]
  *   and out[M, N/2] = (x + bx) * gelu_erf(g + bg); act/gate/residual are not applied.
- * conv_mode=1: A is an NHWC activation [B, H, W, C=K] (ld = pixel stride); W is [9][N][K]; zero padding 1.
+ * conv_mode=1: A is an NHWC activation [B, H, W, C=K] (ld = pixel stride); W is [9][N][K]; zero padding 1; any H, W.
  *
  * LayerNorm fold (attention.py:309-311,225-226 nn.LayerNorm feeding a Linear): with W' = W * gamma (per input
  *   channel, folded into W by the caller), colsum[n] = sum_k W'[n,k] and bias' = bias + W beta,
