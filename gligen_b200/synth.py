@@ -10,7 +10,7 @@ invalid -> (0,0) and mask = (mean != 0) (gligen_inference.py:199-218).
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple, Union
 
 import torch
 
@@ -18,10 +18,10 @@ from .spec import SPATIAL_MAP_KEY, UNetConfig
 
 
 def make_grounding_batch(cfg: UNetConfig, B: int, max_objs: int, g: torch.Generator,
-                         n_valid: Optional[int] = None) -> Dict[str, torch.Tensor]:
+                         n_valid: Optional[int] = None, map_size: Optional[Tuple[int, int]] = None) -> Dict[str, torch.Tensor]:
     """The `batch` dict handed to GroundingNetInput.prepare (gligen_inference.py:411)."""
     if cfg.spatial:
-        return make_spatial_batch(cfg, B, g)
+        return make_spatial_batch(cfg, B, g, map_size)
     if cfg.tokenizer == "keypoint":
         n = cfg.max_persons * 17
         pts = torch.rand(B, n, 2, generator=g)
@@ -47,22 +47,27 @@ def make_grounding_batch(cfg: UNetConfig, B: int, max_objs: int, g: torch.Genera
     return out
 
 
-def make_spatial_batch(cfg: UNetConfig, B: int, g: torch.Generator, size: Optional[int] = None) -> Dict[str, torch.Tensor]:
-    """A spatial conditioning map at twice the tokenizer's input size (512 x 512 for the shipped configs) the way the datasets
-    deliver it: grey maps (hed / canny / depth) replicated to 3 channels in [0, 1], normals in [-1, 1], semantic maps one-hot
-    over `sem_in_dim` classes; `mask` = 1 (map present; the null input is a zero map with mask 0)."""
+def make_spatial_batch(cfg: UNetConfig, B: int, g: torch.Generator,
+                       size: Optional[Union[int, Tuple[int, int]]] = None) -> Dict[str, torch.Tensor]:
+    """A spatial conditioning map of `size` = side or (H, W), by default square at twice the tokenizer's input size (512 x 512
+    for the shipped configs), the way the datasets deliver it: grey maps (hed / canny / depth) replicated to 3 channels in
+    [0, 1], normals in [-1, 1], semantic maps one-hot over `sem_in_dim` classes in constant label blocks; `mask` = 1 (map
+    present; the null input is a zero map with mask 0).  Square maps use 16-pixel blocks; non-square ones use 13-pixel
+    blocks, which no resampling ratio of theirs lines up with, so an off-by-one source index changes the labels it reads."""
     size = size or 2 * cfg.tok_resize
+    H, W = (size, size) if isinstance(size, int) else size
     key = SPATIAL_MAP_KEY[cfg.tokenizer]
     if cfg.tokenizer == "sem":
-        coarse = torch.randint(0, cfg.sem_in_dim, (B, size // 16, size // 16), generator=g)
-        labels = coarse.repeat_interleave(16, 1).repeat_interleave(16, 2)
+        blk = 16 if H == W else 13
+        coarse = torch.randint(0, cfg.sem_in_dim, (B, -(-H // blk), -(-W // blk)), generator=g)
+        labels = coarse.repeat_interleave(blk, 1).repeat_interleave(blk, 2)[:, :H, :W]
         m = torch.nn.functional.one_hot(labels, cfg.sem_in_dim).permute(0, 3, 1, 2).float().contiguous()
     elif cfg.tokenizer == "normal":
-        m = torch.rand(B, 3, size, size, generator=g) * 2 - 1
+        m = torch.rand(B, 3, H, W, generator=g) * 2 - 1
     else:
-        base = torch.rand(B, 1, size, size, generator=g)
+        base = torch.rand(B, 1, H, W, generator=g)
         if cfg.tokenizer in ("hed", "canny"):
-            base = (base > 0.8).float() * torch.rand(B, 1, size, size, generator=g)       # sparse edge responses
+            base = (base > 0.8).float() * torch.rand(B, 1, H, W, generator=g)       # sparse edge responses
         m = base.repeat(1, 3, 1, 1).contiguous()
     return {key: m, "mask": torch.ones(B)}
 
@@ -79,8 +84,8 @@ def grounding_kwargs(cfg: UNetConfig, batch: Dict[str, torch.Tensor]) -> Dict[st
 
 
 def make_inputs(cfg: UNetConfig, B: int, max_objs: int = 30, seed: int = 2, n_valid: Optional[int] = None,
-                n_ctx: int = 77) -> Dict[str, object]:
-    """x_T, context, uc, grounding batch (+ inpainting tensors when cfg.inpaint_mode)."""
+                n_ctx: int = 77, map_size: Optional[Tuple[int, int]] = None) -> Dict[str, object]:
+    """x_T, context, uc, grounding batch (+ inpainting tensors when cfg.inpaint_mode); `map_size` (H, W): the spatial map's."""
     g = torch.Generator(device="cpu").manual_seed(seed)
     hw = cfg.image_size
     out: Dict[str, object] = {
@@ -88,7 +93,7 @@ def make_inputs(cfg: UNetConfig, B: int, max_objs: int = 30, seed: int = 2, n_va
         "context": torch.randn(B, n_ctx, cfg.context_dim, generator=g),
         "uc": torch.randn(B, n_ctx, cfg.context_dim, generator=g),
     }
-    batch = make_grounding_batch(cfg, B, max_objs, g, n_valid)
+    batch = make_grounding_batch(cfg, B, max_objs, g, n_valid, map_size)
     out["batch"] = batch
     out["grounding_input"] = grounding_kwargs(cfg, batch)
     if cfg.spatial:          # GroundingDSInput.prepare (grounding_input/*_grounding_downsampler_input.py:16): the same map

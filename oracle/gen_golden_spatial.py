@@ -32,7 +32,8 @@ GOLD = os.path.join(REPO, "tests", "golden")
 TS = [981, 501]
 
 
-def run(name: str, B: int, seed: int, plms: bool = False) -> None:
+def run(name: str, B: int, seed: int, plms: bool = False, map_size=None) -> None:
+    """Writes spatial_{name}.pt, or spatial_{name}_{H}x{W}.pt for a map of `map_size` (H, W) instead of the default square one."""
     cfg = NAMED_CONFIGS[name]
     t0 = time.time()
     sd = synthetic_state_dict(cfg, 0)
@@ -41,7 +42,7 @@ def run(name: str, B: int, seed: int, plms: bool = False) -> None:
     missing, unexpected = model.load_state_dict(sd, strict=True)
     assert not missing and not unexpected
     model.grounding_tokenizer_input = RH.ref_grounding_input(cfg)
-    inp = synth.make_inputs(cfg, B, seed=seed)
+    inp = synth.make_inputs(cfg, B, seed=seed, map_size=map_size)
     batch = inp["batch"]
     grounding = model.grounding_tokenizer_input.prepare(batch)
     ts = torch.tensor(TS[:B])
@@ -72,9 +73,13 @@ def run(name: str, B: int, seed: int, plms: bool = False) -> None:
         lat, secs = RH.run_reference_sampler(cfg, sd, inp, "plms", 4, [0.5, 0.0, 0.5], guidance=5.0, verbose=False)
         extra["plms"] = {"S": 4, "alpha_type": [0.5, 0.0, 0.5], "guidance": 5.0, "latent": lat.clone()}
         print(f"{name}: reference PLMS S=4 [0.5,0,0.5] latent std {lat.std():.3f} ({secs:.1f} s)", flush=True)
+    shape = tuple(inp["grounding_extra_input"].shape[2:])
+    print(f"{name}: map {shape[0]} x {shape[1]}", flush=True)
+    tag = "" if map_size is None else f"_{map_size[0]}x{map_size[1]}"
     torch.save({"config": name, **extra, "B": B, "seed": seed, "timesteps": TS[:B], "map_key": SPATIAL_MAP_KEY[cfg.tokenizer],
+                **({} if map_size is None else {"map_size": shape}),
                 "oracle_vs_reference_max_abs": errs, **{k: v.clone() for k, v in out.items()}},
-               os.path.join(GOLD, f"spatial_{name}.pt"))
+               os.path.join(GOLD, f"spatial_{name}{tag}.pt"))
 
 
 if __name__ == "__main__":
@@ -86,6 +91,11 @@ if __name__ == "__main__":
     for name in ("tiny_hed", "tiny_canny", "tiny_depth", "tiny_normal", "tiny_sem"):
         if only is None or name in only.split(","):
             run(name, 2, 11)
+    # non-square maps (a 3:5 landscape and a 4:3 portrait): bicubic only (hed), bicubic + conv (normal), nearest fused into the
+    # convolutions (sem); every resampling ratio there is not an integer and differs between the axes
+    for name, size in (("tiny_hed", (192, 320)), ("tiny_normal", (300, 224)), ("tiny_sem", (300, 224))):
+        if only is None or f"{name}_{size[0]}x{size[1]}" in only.split(","):
+            run(name, 2, 11, map_size=size)
     if a.full:
         for name in ("sd14_hed", "sd14_sem"):
             run(name, 1, 12, plms=(name == "sd14_hed"))

@@ -3,9 +3,10 @@
 CheckedOps wraps CudaOps: each call snapshots its inputs (the residual is often the output itself), runs the kernel,
 synchronises and checks the output against RefOps(float64) on the snapshot - the GEMM family and attention with the
 rounding-level bounds of tests/bounds.py, GroupNorm, the LayerNorms, softmax_rows and the edge convolutions with
-the bounds derived for them there, as are the embeddings, token rows, dwconv7_ln, the CLIP vision embed / head and the
-sampler update; stats_out bit for bit against its documented summation order; cast and the copies exactly; the
-fp32 resampling ops of the spatial modalities at the tolerances of tests/test_spatial_gpu.py.  The forwards run with seeded synthetic weights and no CUDA graphs, so
+the bounds derived for them there, as are the embeddings, token rows, dwconv7_ln, the CLIP vision embed / head, the
+sampler update, and the resampling ops of the spatial modalities (resize_plane, conv2d_small) with the bounds of
+tests/bounds_resample.py; stats_out bit for bit
+against its documented summation order; cast, the copies and the patch gathers exactly.  The forwards run with seeded synthetic weights and no CUDA graphs, so
 every call of the plan is seen.  A failure lists every violating call with its shapes, strides, flags and tile choice."""
 import ctypes as C
 import inspect
@@ -15,16 +16,16 @@ import pytest
 import torch
 
 import bounds
+import bounds_resample
 from conftest import assert_close
 from ref_ops import RefOps
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
-# outputs of the ops still checked at the kernel suite's tolerances: name -> (output arguments, rel-L2, max-rel)
+# outputs of the ops that move values without arithmetic, checked bit for bit: name -> (output arguments, rel-L2, max-rel)
 SMALL_OPS = {
     "cast": (("y",), 0.0, 0.0), "upsample2x": (("y",), 0.0, 0.0), "im2col_s2": (("y",), 0.0, 0.0),
-    "resize_plane": (("y",), 2e-3, 5e-3), "conv2d_small": (("y",), 2e-3, 5e-3),
     "patchify_nchw": (("out",), 0.0, 0.0), "patchify_nhwc": (("out",), 0.0, 0.0),
 }
 
@@ -188,6 +189,19 @@ class CheckedOps:
         torch.cuda.synchronize()
         self._record("clip_image_head", bounds.clip_image_head_check(pooled, embeds, x, gamma, beta, w_proj, eps))
 
+    def resize_plane(self, x, y, C, mode):
+        x0 = x.clone()
+        self.inner.resize_plane(x, y, C, mode)
+        torch.cuda.synchronize()
+        self._record("resize_plane", bounds_resample.resize_check(y, x0, mode, what=f"resize_plane x={_desc(x)} y={_desc(y)} {mode}"))
+
+    def conv2d_small(self, x, w, bias, y, k, stride, pad, silu, virtual=None):
+        x0 = x.clone()
+        self.inner.conv2d_small(x, w, bias, y, k, stride, pad, silu, virtual=virtual)
+        torch.cuda.synchronize()
+        what = f"conv2d_small x={_desc(x)} y={_desc(y)} k={k} stride={stride} pad={pad} silu={silu} virtual={virtual}"
+        self._record("conv2d_small", bounds_resample.conv2d_small_check(y, x0, w, bias, k, stride, pad, silu, virtual, what=what))
+
     def _small(self, name, fn, *a, **kw):
         outs, rel, max_rel = SMALL_OPS[name]
         bound = inspect.signature(getattr(RefOps, name)).bind(None, *a, **kw)
@@ -230,7 +244,7 @@ def cuda_ops():
     return CudaOps(DEV)
 
 
-def _unet_forward(cuda_ops, name, B, cfg_batch):
+def _unet_forward(cuda_ops, name, B, cfg_batch, map_size=None):
     from gligen_b200 import synth
     from gligen_b200.engine import Engine
     from gligen_b200.spec import NAMED_CONFIGS, SPATIAL_MAP_KEY, synthetic_state_dict
@@ -239,7 +253,7 @@ def _unet_forward(cuda_ops, name, B, cfg_batch):
     ops = CheckedOps(cuda_ops)
     eng = Engine(cfg, ops, use_graphs=False)
     eng.load_state_dict(synthetic_state_dict(cfg, 0))
-    inp = synth.make_inputs(cfg, B, seed=2)
+    inp = synth.make_inputs(cfg, B, seed=2, map_size=map_size)
     x, ctx, uc = (inp[k].to(DEV) for k in ("x", "context", "uc"))
     ts = torch.tensor([981, 501, 21, 700][:B] * (B // 4 + 1), device=DEV)[:B]
     gr = {k: v.to(DEV) for k, v in inp["grounding_input"].items()}
@@ -254,7 +268,7 @@ def _unet_forward(cuda_ops, name, B, cfg_batch):
     else:
         eng.forward(x, ts, ctx, gr, extra, gextra)
     torch.cuda.synchronize()
-    _summary(f"{name} B={B}{' cfg' if cfg_batch else ''}", ops)
+    _summary(f"{name} B={B}{' cfg' if cfg_batch else ''}{f' map {map_size[0]}x{map_size[1]}' if map_size else ''}", ops)
 
 
 def test_census_sd14_box_text_cfg_b4(cuda_ops):
@@ -275,6 +289,13 @@ def _tiny_names():
 @pytest.mark.parametrize("name", _tiny_names())
 def test_census_tiny(cuda_ops, name):
     _unet_forward(cuda_ops, name, 2, True)
+
+
+@pytest.mark.parametrize("name,map_size", [("tiny_hed", (192, 320)), ("tiny_normal", (300, 224)), ("tiny_sem", (300, 224)),
+                                           ("tiny_depth", (480, 640))])
+def test_census_tiny_non_square_map(cuda_ops, name, map_size):
+    """The spatial front end on non-square maps: resampling ratios that are not integers and differ between the axes."""
+    _unet_forward(cuda_ops, name, 2, True, map_size)
 
 
 def test_census_vae_sd14(cuda_ops):

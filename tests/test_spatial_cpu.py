@@ -18,16 +18,27 @@ from oracle import unet_oracle as UO
 from ref_ops import RefOps
 
 TINY = ["tiny_hed", "tiny_canny", "tiny_depth", "tiny_normal", "tiny_sem"]
+NON_SQUARE = ["tiny_hed_192x320", "tiny_normal_300x224", "tiny_sem_300x224"]       # fixtures of H x W maps
 
 
 def _load(name):
     g = torch.load(os.path.join(GOLD, f"spatial_{name}.pt"))
-    cfg = NAMED_CONFIGS[name]
-    inp = synth.make_inputs(cfg, g["B"], seed=g["seed"])
+    cfg = NAMED_CONFIGS[g["config"]]
+    inp = synth.make_inputs(cfg, g["B"], seed=g["seed"], map_size=g.get("map_size"))
     return cfg, g, inp, torch.tensor(g["timesteps"])
 
 
-@pytest.mark.parametrize("name", TINY)
+@pytest.mark.parametrize("name", NON_SQUARE)
+def test_non_square_fixture(name):
+    """The fixture's map is the non-square one its name says, and the oracle matched the reference on it when it was written."""
+    cfg, g, inp, _ = _load(name)
+    H, W = (int(v) for v in name.rsplit("_", 1)[1].split("x"))
+    assert tuple(g["map_size"]) == (H, W) and H != W
+    assert tuple(inp["grounding_extra_input"].shape[2:]) == (H, W)
+    assert max(g["oracle_vs_reference_max_abs"].values()) <= 2e-4
+
+
+@pytest.mark.parametrize("name", TINY + NON_SQUARE)
 def test_oracle_matches_reference_fixture(name):
     cfg, g, inp, ts = _load(name)
     sd = synthetic_state_dict(cfg, 0)
@@ -39,7 +50,7 @@ def test_oracle_matches_reference_fixture(name):
         assert (got - g[key]).abs().max() <= 2e-5, key
 
 
-@pytest.mark.parametrize("name", TINY)
+@pytest.mark.parametrize("name", TINY + NON_SQUARE)
 def test_engine_plan_matches_reference(name):
     cfg, g, inp, ts = _load(name)
     eng = Engine(cfg, RefOps())

@@ -137,13 +137,16 @@ def test_gemm_gelu_epilogues(ops, ref, act, M, N, K):
 
 
 # ---- the drop-in model against the reference fixtures ------------------------------------------------------------------------------
-def _run(name):
+def _run(name, model=None):
+    """The drop-in model (a fresh one, or `model`) on the inputs of fixture spatial_{name}.pt, against its eps."""
     from gligen_b200 import synth
     from gligen_b200.pipeline import build_model, sampler_inputs, to_device
-    from gligen_b200.spec import NAMED_CONFIGS
     g = torch.load(os.path.join(GOLD, f"spatial_{name}.pt"))
-    cfg, model = build_model(name, device=DEV)
-    inp = synth.make_inputs(cfg, g["B"], seed=g["seed"])
+    if model is None:
+        cfg, model = build_model(g["config"], device=DEV)
+    else:
+        cfg = model.engine().cfg
+    inp = synth.make_inputs(cfg, g["B"], seed=g["seed"], map_size=g.get("map_size"))
     ts = torch.tensor(g["timesteps"], device=DEV)
     dinp = to_device({k: v for k, v in inp.items() if k in ("x", "context", "uc")}, DEV)
     input, _, _ = sampler_inputs(cfg, model, dinp, to_device(inp["batch"], DEV))
@@ -161,9 +164,19 @@ def _run(name):
     return cfg, model, g, inp
 
 
-@pytest.mark.parametrize("name", ["tiny_hed", "tiny_canny", "tiny_depth", "tiny_normal", "tiny_sem"])
+@pytest.mark.parametrize("name", ["tiny_hed", "tiny_canny", "tiny_depth", "tiny_normal", "tiny_sem",
+                                  "tiny_hed_192x320", "tiny_normal_300x224", "tiny_sem_300x224"])
 def test_forward_tiny_spatial(name):
     _run(name)
+
+
+@pytest.mark.parametrize("square,other", [("tiny_hed", "tiny_hed_192x320"), ("tiny_sem", "tiny_sem_300x224")])
+def test_map_size_change_replans(square, other):
+    """One model fed a square map, then a non-square one, then the square one again: each result matches its own fixture,
+    so no plan or static buffer sized for one map survives the change to the other."""
+    _, model, _, _ = _run(square)
+    _run(other, model)
+    _run(square, model)
 
 
 @pytest.mark.parametrize("name", ["sd14_hed", "sd14_sem"])
