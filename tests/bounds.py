@@ -219,26 +219,75 @@ def _matmul_abs(a, w, conv):
     return sum(xp[:, t // 3:t // 3 + H, t % 3:t % 3 + Wd].reshape(-1, K) @ wt[t].t() for t in range(9))
 
 
-def gemm_check(got, a, w, bias=None, rowbias=None, rows_per_batch=1, act=0, gate=None, residual=None, geglu=False,
-               conv=None, ln=None, splits=1, aggregate=True, what="gemm") -> Report:
-    """Bound of the module docstring for one glg_gemm call (arguments as CudaOps.gemm; `got` the stored output)."""
+class _Worst:
+    """The elementwise worst over row chunks, and per-row sums of squares for the aggregate rel-L2.  The sums over all
+    rows are taken once at the end, so a report does not depend on how its rows were chunked."""
+
+    def __init__(self, rows, cols, dev):
+        self.cols = cols
+        self.ratio, self.i, self.vals = -math.inf, 0, (0.0, 0.0)
+        self.sq = torch.zeros(4, rows, dtype=torch.float64, device=dev)  # |got - ref|^2, |ref|^2, |bf16(ref) - ref|^2, stats^2
+
+    def add(self, r0, got64, ref, err, dtype, stats=None, sums=True):
+        """Rows [r0, r0 + len(ref)) of the output ([rows, cols] float64 views; dtype the stored output's)."""
+        ratio, i, _ = _elementwise(got64, ref, err, dtype)
+        if not math.isnan(self.ratio) and not ratio <= self.ratio:         # a NaN ratio is kept
+            self.ratio, self.i = ratio, r0 * self.cols + i
+            self.vals = (got64.reshape(-1)[i].item(), ref.reshape(-1)[i].item())
+        if sums and dtype == torch.bfloat16:
+            rows = slice(r0, r0 + ref.shape[0])
+            self.sq[0, rows] = ((got64 - ref) ** 2).sum(1)
+            self.sq[1, rows] = (ref ** 2).sum(1)
+            self.sq[2, rows] = ((round_to(ref, torch.bfloat16) - ref) ** 2).sum(1)
+            if stats is not None:
+                st = torch.where(torch.isfinite(stats), stats, torch.zeros_like(stats))
+                self.sq[3, rows] = (st ** 2).sum(1)
+
+    def aggregate(self):
+        """(rel-L2 over the limit 1.25 r0 + the rel-L2 of the statistics term, details) for bf16 outputs."""
+        d, nref, d0, st = self.sq.sum(1).sqrt().tolist()
+        nref = max(nref, 1e-300)
+        r, r0, allow = d / nref, d0 / nref, st / nref
+        agg = r / (1.25 * r0 + allow) if r0 > 0 else (0.0 if r == 0 else math.inf)
+        return agg, dict(rel_l2=r, r0=r0)
+
+
+def _row_chunks(rows, cols, max_elems, conv=None):
+    """Row ranges (compute c0, c1, keep k0, k1, conv of the compute rows) such that one float64 [rows, cols] intermediate
+    of a chunk stays within `max_elems` bytes (None: one chunk of every row).  A 3x3 convolution is chunked by whole
+    image rows and computes one halo row above and below each chunk (kept rows only are checked), so every kept output
+    sees the same taps and zero padding as in the whole image."""
+    if max_elems is None:
+        yield 0, rows, 0, rows, conv
+        return
+    if conv is None:
+        step = max(1, max_elems // (8 * cols))
+        for r in range(0, rows, step):
+            yield r, min(rows, r + step), r, min(rows, r + step), None
+        return
+    B, H, Wd = conv
+    step = max(1, max_elems // (8 * cols * Wd))
+    for b in range(B):
+        for y0 in range(0, H, step):
+            y1 = min(H, y0 + step)
+            ys, ye = max(0, y0 - 1), min(H, y1 + 1)
+            base = b * H * Wd
+            yield base + ys * Wd, base + ye * Wd, base + y0 * Wd, base + y1 * Wd, (1, ye - ys, Wd)
+
+
+def _gemm_rows(a, w, bias, rowbias, act, gate, residual, geglu, conv, ln, gamma):
+    """(ref, error bound, LayerNorm-statistics part) of the GEMM rows a [M, K] (rowbias already one row per output row)."""
     from ref_ops import RefOps
     f64 = torch.float64
-    dev = got.device
-    M = got.numel() // got.shape[-1]
-    Nout = got.shape[-1]
-    ref = torch.empty(got.shape, dtype=f64, device=dev)
-    RefOps(dev, compute_dtype=f64).gemm(a, w, ref, bias=bias, rowbias=rowbias, rows_per_batch=rows_per_batch, act=act,
-                                        gate=gate, residual=residual, geglu=geglu, conv=conv, ln=ln)
-    ref = ref.reshape(M, Nout)
-    got64 = got.reshape(M, Nout).to(f64)
-    K = a.shape[-1]
-    ktot = K * (9 if conv is not None else 1)
-    gamma = 17.0 / 16.0 * ktot * T + (splits + 4) * U
+    dev = a.device
+    M, K = a.shape
+    ref64 = RefOps(dev, compute_dtype=f64)
+    N = w.shape[0] // (9 if conv is not None else 1)
+    Nout = N // 2 if geglu else N
+    ref = torch.empty(M, Nout, dtype=f64, device=dev)
+    ref64.gemm(a, w, ref, bias=bias, rowbias=rowbias, act=act, gate=gate, residual=residual, geglu=geglu, conv=conv, ln=ln)
     S = _matmul_abs(a, w, conv)                                   # [M, N]
-    N = S.shape[1]
     extra = torch.zeros_like(S)                                   # LayerNorm-statistics error (not scaled by gamma)
-    y_pre_abs = None
     if ln is not None:
         st, colsum, eps = ln
         st = st.to(f64)
@@ -253,19 +302,18 @@ def gemm_check(got, a, w, bias=None, rowbias=None, rows_per_batch=1, act=0, gate
         dvar = (slots + 2) * U * ex2 + 2 * mu.abs() * dmu + U * mu * mu + U * (var + eps)
         drel = dvar / (2 * (var + eps)) + 2 * T
         cs = colsum.to(f64)
-        A = a.reshape(-1, K).to(f64)
+        A = a.to(f64)
         y_ln = rstd[:, None] * (A @ w.to(f64).t() - mu[:, None] * cs[None])
         S = rstd[:, None] * (S + mu.abs()[:, None] * cs.abs()[None])
         extra = drel[:, None] * y_ln.abs() + (rstd * dmu)[:, None] * cs.abs()[None]
     if bias is not None:
         S = S + bias.to(f64).abs()[None]
     if rowbias is not None:
-        idx = torch.arange(M, device=dev) // rows_per_batch
-        S = S + rowbias.to(f64).abs()[idx]
+        S = S + rowbias.to(f64).abs()
     e = gamma * S + extra                                         # error of the pre-activation value
     if geglu:
         pre = torch.empty(M, N, dtype=f64, device=dev)
-        RefOps(dev, compute_dtype=f64).gemm(a, w, pre, bias=bias, ln=ln)
+        ref64.gemm(a, w, pre, bias=bias, ln=ln)
         t4 = pre.view(M, N // 256, 2, 128)
         x, g = t4[:, :, 0], t4[:, :, 1]
         e4 = e.view(M, N // 256, 2, 128)
@@ -276,46 +324,62 @@ def gemm_check(got, a, w, bias=None, rowbias=None, rows_per_batch=1, act=0, gate
         err = e
         if act:
             pre = torch.empty(M, N, dtype=f64, device=dev)
-            RefOps(dev, compute_dtype=f64).gemm(a, w, pre, bias=bias, rowbias=rowbias, rows_per_batch=rows_per_batch, ln=ln)
+            ref64.gemm(a, w, pre, bias=bias, rowbias=rowbias, ln=ln)
             post = ref if (gate is None and residual is None) else torch.empty_like(pre)
             if post is not ref:
-                RefOps(dev, compute_dtype=f64).gemm(a, w, post, bias=bias, rowbias=rowbias, rows_per_batch=rows_per_batch, act=act, ln=ln)
+                ref64.gemm(a, w, post, bias=bias, rowbias=rowbias, act=act, ln=ln)
             own = EPS_GELU + 4 * U * pre.abs() if act == 2 else (5 + 2.5 * pre.abs()) * T * post.abs()
             err = ACT_SLOPE * err + own
         if gate is not None:
             gv = float(gate.reshape(-1)[0])
             err = abs(gv) * err + U * (ref.abs() + err)
         if residual is not None:
-            err = err + U * (ref.abs() + residual.reshape(M, -1).to(f64).abs() + err)
+            err = err + U * (ref.abs() + residual.to(f64).abs() + err)
+    return ref, err, extra
+
+
+def gemm_check(got, a, w, bias=None, rowbias=None, rows_per_batch=1, act=0, gate=None, residual=None, geglu=False,
+               conv=None, ln=None, splits=1, aggregate=True, what="gemm", max_elems=None) -> Report:
+    """Bound of the module docstring for one glg_gemm call (arguments as CudaOps.gemm; `got` the stored output).
+    max_elems: evaluate in row chunks whose float64 [rows, max(N, K)] intermediates stay within that many bytes (None:
+    all rows at once).  The report is the same either way."""
+    f64 = torch.float64
+    dev = got.device
+    M = got.numel() // got.shape[-1]
+    Nout = got.shape[-1]
+    K = a.shape[-1]
+    ktot = K * (9 if conv is not None else 1)
+    gamma = 17.0 / 16.0 * ktot * T + (splits + 4) * U
+    A, G = a.reshape(-1, K), got.reshape(M, Nout)
+    R = None if residual is None else residual.reshape(M, -1)
     dt = got.dtype
-    ratio, i, _ = _elementwise(got64, ref, err, dt)
-    agg = 0.0
-    ex = {}
-    if dt == torch.bfloat16 and aggregate:
-        r0 = rel_l2(round_to(ref, torch.bfloat16), ref)
-        allow = (extra.norm() / ref.norm().clamp_min(1e-300)).item() if ln is not None else 0.0
-        r = rel_l2(got64, ref)
-        agg = r / (1.25 * r0 + allow) if r0 > 0 else (0.0 if r == 0 else math.inf)
-        ex = dict(rel_l2=r, r0=r0)
-    row, col = divmod(i, Nout)
-    worst = f"(worst at row {row} col {col}: got {got64.reshape(-1)[i].item():.6g} ref {ref.reshape(-1)[i].item():.6g})"
-    return Report(what, ratio, agg, worst, ex)
+    acc = _Worst(M, Nout, dev)
+    for c0, c1, k0, k1, cv in _row_chunks(M, max(w.shape[0] // (9 if conv is not None else 1), K), max_elems, conv):
+        rb = None if rowbias is None else rowbias[torch.arange(c0, c1, device=rowbias.device) // rows_per_batch]
+        lnc = None if ln is None else (ln[0][:, c0:c1], ln[1], ln[2])
+        ref, err, extra = _gemm_rows(A[c0:c1], w, bias, rb, act, gate, None if R is None else R[c0:c1], geglu, cv, lnc, gamma)
+        keep = slice(k0 - c0, k1 - c0)
+        acc.add(k0, G[k0:k1].to(f64), ref[keep], err[keep], dt, extra[keep] if ln is not None else None, sums=aggregate)
+    agg, ex = acc.aggregate() if dt == torch.bfloat16 and aggregate else (0.0, {})
+    row, col = divmod(acc.i, Nout)
+    worst = f"(worst at row {row} col {col}: got {acc.vals[0]:.6g} ref {acc.vals[1]:.6g})"
+    return Report(what, acc.ratio, agg, worst, ex)
 
 
 def _heads(t, B, L, H, d):
     return t.reshape(B, L, H, d).permute(0, 2, 1, 3).to(torch.float64)
 
 
-def attention_check_scores(got, s, v, c, d, poly=0, causal=False, qk_abs=None, what="attention") -> Report:
+def attention_check_scores(got, s, v, c, d, poly=0, causal=False, qk_abs=None, what="attention", row0=0) -> Report:
     """Bound for outputs `got` [n, Lq, dv] of rows with exact scores s [n, Lq, Lk] (fp64, before the scale), values
     v [n, Lk, dv] and exponent scale c (scale * log2 e).  qk_abs [n, Lq, Lk] = sum|q||k| (None: scores are exact inputs,
-    d products per score otherwise)."""
+    d products per score otherwise).  row0: query index of the first row (the causal mask and the report)."""
     f64 = torch.float64
     n, Lq, Lk = s.shape
     s = s.to(f64)
     v = v.to(f64)
     if causal:
-        s = s.masked_fill(torch.ones(Lq, Lk, dtype=torch.bool, device=s.device).triu(1), float("-inf"))
+        s = s.masked_fill(torch.ones(Lq, Lk, dtype=torch.bool, device=s.device).triu(1 + row0), float("-inf"))
     ntiles = (Lk + 63) // 64
     pad = ntiles * 64 - Lk
     sp = torch.nn.functional.pad(s, (0, pad), value=float("-inf"))
@@ -354,7 +418,7 @@ def attention_check_scores(got, s, v, c, d, poly=0, causal=False, qk_abs=None, w
     dv = o.shape[-1]
     hq, col = divmod(i, dv)
     hh, row = divmod(hq, Lq)
-    return Report(what, ratio, 0.0, f"(worst at row {row} col {col} of slice {hh}: got {got64.reshape(-1)[i].item():.6g} "
+    return Report(what, ratio, 0.0, f"(worst at row {row0 + row} col {col} of slice {hh}: got {got64.reshape(-1)[i].item():.6g} "
                                     f"ref {o.reshape(-1)[i].item():.6g})")
 
 
@@ -368,7 +432,8 @@ def _spread(wr, v, o):
 
 
 def attention_check(got, q, k, v, heads, d_head, poly=0, causal=False, what="attention", max_elems=2 ** 28) -> Report:
-    """Bound for one glg_attention call (arguments as CudaOps.attention), in fp64 chunks of batch x heads."""
+    """Bound for one glg_attention call (arguments as CudaOps.attention), in fp64 chunks of batch x heads, and of query
+    rows when one head's [Lq, Lk] scores exceed max_elems bytes."""
     B, Lq, _ = q.shape
     Lk = k.shape[1]
     scale = float(d_head) ** -0.5
@@ -376,16 +441,19 @@ def attention_check(got, q, k, v, heads, d_head, poly=0, causal=False, what="att
     worst = Report(what, 0.0)
     G = B * heads
     per = max(1, max_elems // (Lq * Lk * 8))
+    rows = max(1, min(Lq, max_elems // (Lk * 8)))
     qh, kh, vh = _heads(q, B, Lq, heads, d_head), _heads(k, B, Lk, heads, d_head), _heads(v, B, Lk, heads, d_head)
     gh = _heads(got, B, Lq, heads, d_head)
     qh, kh, vh, gh = (t.reshape(G, t.shape[2], d_head) for t in (qh, kh, vh, gh))
     for g0 in range(0, G, per):
         sl = slice(g0, g0 + per)
-        s = qh[sl] @ kh[sl].transpose(1, 2)
-        qk = qh[sl].abs() @ kh[sl].abs().transpose(1, 2)
-        rep = attention_check_scores(gh[sl], s, vh[sl], c, d_head, poly=poly, causal=causal, qk_abs=qk, what=what)
-        if rep.ratio > worst.ratio:
-            worst = rep
+        for r0 in range(0, Lq, rows):
+            rs = slice(r0, r0 + rows)
+            s = qh[sl, rs] @ kh[sl].transpose(1, 2)
+            qk = qh[sl, rs].abs() @ kh[sl].abs().transpose(1, 2)
+            rep = attention_check_scores(gh[sl, rs], s, vh[sl], c, d_head, poly=poly, causal=causal, qk_abs=qk, what=what, row0=r0)
+            if not math.isnan(worst.ratio) and not rep.ratio <= worst.ratio:     # a NaN ratio is kept
+                worst = rep
     return worst
 
 
@@ -586,25 +654,31 @@ def layernorm_check(y, x, gamma, beta, eps, what="layernorm", x_err=None, depth=
     return _finish(y, ref, err, stats, what, lambda i: f"row {i // C} col {i % C}")
 
 
-def softmax_check(p, s, scale, what="softmax_rows") -> Report:
-    """Bound for one glg_softmax_rows call: s fp32 [rows, cols], p bf16 [rows, cols]."""
+def softmax_check(p, s, scale, what="softmax_rows", max_elems=None) -> Report:
+    """Bound for one glg_softmax_rows call: s fp32 [rows, cols], p bf16 [rows, cols].  max_elems: as gemm_check's, row
+    chunks whose float64 [rows, cols] intermediates stay within that many bytes (None: all rows at once)."""
     f64 = torch.float64
     rows, cols = s.shape
-    s64 = s.to(f64)
     c = scale * 1.4426950408889634
-    m = s64.amax(1, keepdim=True)
-    x = (s64 - m) * c
-    e = torch.exp2(x)
-    ref = e / e.sum(1, keepdim=True)
-    r = LN2 * (U * (m * c).abs() + U * x.abs() + 3 * U * x.abs()) + 2 * T
-    tiny = 2.0 ** -148 / e.clamp_min(2.0 ** -1074)
-    r = r + torch.where(e < 2.0 ** -126, tiny, torch.zeros_like(tiny))
     L = 3 + -(-cols // 1024) + 13
-    tau = g_n(L) * (1 + r.amax(1, keepdim=True)) + (r * e).sum(1, keepdim=True) / e.sum(1, keepdim=True)
-    rel = (1 + r) * (1 + U) ** 2 / (1 - tau) - 1
-    err = (ref * rel).clamp_max(1.0)
-    err = err + 2.0 ** -149 * 2                                                   # the subnormal range of the fp32 product
-    return _finish(p, ref, err, torch.zeros_like(ref), what, lambda i: f"row {i // cols} col {i % cols}")
+    acc = _Worst(rows, cols, s.device)
+    for r0, r1, _, _, _ in _row_chunks(rows, cols, max_elems):
+        s64 = s[r0:r1].to(f64)
+        m = s64.amax(1, keepdim=True)
+        x = (s64 - m) * c
+        e = torch.exp2(x)
+        ref = e / e.sum(1, keepdim=True)
+        r = LN2 * (U * (m * c).abs() + U * x.abs() + 3 * U * x.abs()) + 2 * T
+        tiny = 2.0 ** -148 / e.clamp_min(2.0 ** -1074)
+        r = r + torch.where(e < 2.0 ** -126, tiny, torch.zeros_like(tiny))
+        tau = g_n(L) * (1 + r.amax(1, keepdim=True)) + (r * e).sum(1, keepdim=True) / e.sum(1, keepdim=True)
+        rel = (1 + r) * (1 + U) ** 2 / (1 - tau) - 1
+        err = (ref * rel).clamp_max(1.0)
+        err = err + 2.0 ** -149 * 2                                               # the subnormal range of the fp32 product
+        acc.add(r0, p[r0:r1].to(f64), ref, err, p.dtype)
+    agg, ex = acc.aggregate() if p.dtype == torch.bfloat16 else (0.0, {})
+    worst = f"(worst at row {acc.i // cols} col {acc.i % cols}: got {acc.vals[0]:.6g} ref {acc.vals[1]:.6g})"
+    return Report(what, acc.ratio, agg, worst, ex)
 
 
 def conv_check(got, x, w, bias, kind, H=None, W=None, extra=None, what=None) -> Report:

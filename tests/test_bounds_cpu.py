@@ -103,7 +103,7 @@ def attn_restated(s, v, c, Lk, poly=0, mutant=None, exp_poly=ex2_poly3):
     keys = torch.arange(64)
     lane = keys // 8
     cut = Lk + 1 if mutant == "mask_under" else Lk - 1 if mutant == "mask_over" else Lk
-    for kt in range(nkt):
+    for kt in range(nkt - 1 if mutant == "drop_last_tile" else nkt):
         sc = sp[:, kt * 64:(kt + 1) * 64].clone()
         sc[:, kt * 64 + keys >= cut] = -math.inf
         mn = torch.maximum(m, sc.max(1).values)
@@ -161,6 +161,23 @@ def test_attention_mask_over_rejected():
     assert not rep.ok, str(rep)
 
 
+@pytest.mark.parametrize("std,lift", [(1.0, 8.0), (10.0, 0.0)])
+def test_attention_fuser_length_drop_last_tile_rejected(std, lift):
+    """The fuser's key length at a 768^2 image: T = 9216 visual tokens + 30 grounding tokens, so the last 64-key tile
+    holds only the 30 grounding keys.  The faithful restatement passes; one that stops before that ragged tile fails.
+    With logits of std 1 the grounding keys score `lift` above the visual ones (5 % of the softmax mass): 30 keys of
+    equal weight among 9246 move the output less than the P.V accumulation term of the bound."""
+    rows, Lk, c = 16, 9216 + 30, 0.5
+    s = _scores_row_tiles(rows, Lk, std, 13)
+    s[:, 9216:] += lift
+    v = torch.randn(Lk, 16, generator=torch.Generator().manual_seed(14)).to(BF)
+    good = _check_attn(attn_restated(s, v, c, Lk), s, v, c, 0)
+    assert good.ok, str(good)
+    bad = _check_attn(attn_restated(s, v, c, Lk, mutant="drop_last_tile"), s, v, c, 0)
+    print(good, bad)
+    assert not bad.ok, str(bad)
+
+
 @pytest.mark.parametrize("mutant", ["l_not_rescaled", "corr_row8"])
 def test_attention_rescale_mutants_rejected(mutant):
     """Logits of std 10 whose level rises from tile to tile: corr is far from 1 and differs between rows."""
@@ -198,3 +215,82 @@ def test_attention_exp2_twice_the_error_rejected():
     bad = _check_attn(attn_restated(s, v, c, Lk, poly, exp_poly=ex2_poly3_doubled), s, v, c, poly)
     print(good, bad)
     assert not bad.ok, str(bad)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+def _gemm_case(case):
+    """(stored output, gemm_check kwargs, [rows, max(N, K)] columns) of one small GEMM of each epilogue family."""
+    g = torch.Generator().manual_seed(len(case))
+    B, H, Wd, K, N = 2, 5, 7, 64, 32
+    M = B * H * Wd
+    a = torch.randn(M, K, generator=g).to(BF)
+    kw = dict(bias=torch.randn(N, generator=g))
+    if case == "conv":
+        w = (torch.randn(9 * N, K, generator=g) * (9 * K) ** -0.5).to(BF)
+        kw.update(rowbias=torch.randn(B, N, generator=g), rows_per_batch=H * Wd, residual=torch.randn(M, N, generator=g).to(BF),
+                  conv=(B, H, Wd))
+    elif case == "geglu":
+        w = (torch.randn(512, K, generator=g) * K ** -0.5).to(BF)
+        kw.update(bias=torch.randn(512, generator=g), geglu=True)
+    else:
+        w = (torch.randn(N, K, generator=g) * K ** -0.5).to(BF)
+        if case == "ln":
+            kw.update(ln=(bounds.stats_restated(a), w.float().sum(1), 1e-5))
+        elif case == "act":
+            kw.update(act=1, gate=torch.tensor([0.7]), residual=torch.randn(M, N, generator=g).to(BF),
+                      rowbias=torch.randn(7, N, generator=g), rows_per_batch=10)
+    out = torch.empty(M, w.shape[0] // (9 if case == "conv" else 2 if case == "geglu" else 1), dtype=F32 if case == "fp32" else BF)
+    o32 = torch.empty(out.shape)
+    RefOps().gemm(a, w, o32, **kw)
+    out.copy_(o32 + 0.01 * torch.randn(o32.shape, generator=g) * (o32.abs() > 1).float())   # a few elements off their bound
+    return out, a, w, kw
+
+
+def _same_report(a, b):
+    """The same worst element and ratio, bit for bit; the aggregates are float64 sums over per-row partials and may
+    differ in their last bits when a chunk is a single row (torch reduces one row in another order)."""
+    assert (a.ratio, a.worst) == (b.ratio, b.worst)
+    assert math.isclose(a.agg_ratio, b.agg_ratio, rel_tol=1e-13)
+    assert a.extra.keys() == b.extra.keys() and all(math.isclose(a.extra[k], b.extra[k], rel_tol=1e-13) for k in a.extra)
+
+
+@pytest.mark.parametrize("case", ["plain", "fp32", "conv", "ln", "geglu", "act"])
+@pytest.mark.parametrize("max_elems", [1, 8 * 64 * 7 * 2, 8 * 64 * 13])
+def test_gemm_check_chunked_equals_unchunked(case, max_elems):
+    """Row chunks (one row, two image rows of a 3x3 convolution with their halo, 13 rows) report exactly what the
+    whole-matrix evaluation reports: the worst element, its ratio and the aggregate."""
+    out, a, w, kw = _gemm_case(case)
+    whole = bounds.gemm_check(out, a, w, splits=8, **kw)
+    chunked = bounds.gemm_check(out, a, w, splits=8, max_elems=max_elems, **kw)
+    print(whole)
+    _same_report(chunked, whole)
+    assert not whole.ok                                                   # the perturbed elements are found either way
+
+
+@pytest.mark.parametrize("max_elems", [1, 8 * 100 * 3])
+def test_softmax_check_chunked_equals_unchunked(max_elems):
+    import test_bounds_norm_cpu as N
+    g = torch.Generator().manual_seed(4)
+    s = torch.randn(21, 100, generator=g) * 8
+    p = N.softmax_restated(s, 0.25)
+    p[7, 3] = p[7, 3] * 1.1
+    whole, chunked = bounds.softmax_check(p, s, 0.25), bounds.softmax_check(p, s, 0.25, max_elems=max_elems)
+    print(whole)
+    _same_report(chunked, whole)
+    assert not whole.ok
+
+
+@pytest.mark.parametrize("causal", [False, True])
+def test_attention_check_row_chunks_equal_whole(causal):
+    """Query-row chunks of one head (and the causal mask offset by the chunk's first row) report what one chunk does."""
+    g = torch.Generator().manual_seed(5)
+    B, heads, d, L = 1, 2, 16, 90
+    q, k, v = (torch.randn(B, L, heads * d, generator=g).to(BF) for _ in range(3))
+    out = torch.empty(B, L, heads * d, dtype=BF)
+    RefOps().attention(q, k, v, out, heads, d, causal=causal)
+    out[0, 50, 3] = out[0, 50, 3] + 0.05
+    whole = bounds.attention_check(out, q, k, v, heads, d, causal=causal)
+    chunked = bounds.attention_check(out, q, k, v, heads, d, causal=causal, max_elems=8 * L * 7)
+    print(whole)
+    assert (chunked.ratio, chunked.worst) == (whole.ratio, whole.worst)
+    assert not whole.ok and "row 50 col 3 of slice 0" in whole.worst

@@ -292,14 +292,14 @@ def softmax_restated(s, scale, mutant=None):
     """softmax_rows_kernel: thread t owns columns 4 t + 1024 k; exp2f(fmaf(v, c, -m c)); warp_sum; 8 warps in order."""
     R, cols = s.shape
     c = torch.tensor(scale, dtype=F32) * torch.tensor(1.4426950408889634, dtype=F32)
-    m = s.amax(1, keepdim=True)
+    m = (s[:, :4096] if mutant == "stop_4096" else s).amax(1, keepdim=True)
     ms = m * c
     e = torch.exp2(_fma32(s, c.expand_as(s), (-ms).expand_as(s)).to(F64)).to(F32)
     n_k = -(-cols // 1024)
     ep = torch.nn.functional.pad(e, (0, n_k * 1024 - cols)).view(R, n_k, 256, 4)
     acc = torch.zeros(R, 256)
     for k in range(n_k):
-        if mutant == "skip_stride" and k == 1:
+        if mutant == "skip_stride" and k == 1 or mutant == "stop_4096" and k >= 4:     # stop_4096: max and sum loops end at 4096
             continue
         u = ep[:, k]
         acc = acc + (((u[..., 0] + u[..., 1]) + u[..., 2]) + u[..., 3])
@@ -322,6 +322,30 @@ def test_softmax_faithful_passes(cols, std):
     rep = bounds.softmax_check(softmax_restated(s, 0.125), s, 0.125)
     print(rep)
     assert rep.ok, str(rep)
+
+
+@pytest.mark.parametrize("cols", [4100, 9216, 16384])
+def test_softmax_faithful_passes_long_rows(cols):
+    """The VAE mid attention's rows at 768^2 and 1024^2 images (T = 9216, 16384 columns) and one past a 4-column group
+    of 4096; the max in the last 4-column group, and one dominant entry."""
+    g = torch.Generator().manual_seed(cols)
+    s = torch.randn(6, cols, generator=g) * 4
+    s[1, cols - 1] = 60.0
+    s[2, cols - 3] = 400.0
+    rep = bounds.softmax_check(softmax_restated(s, 0.125), s, 0.125)
+    print(rep)
+    assert rep.ok, str(rep)
+
+
+def test_softmax_stop_at_4096_rejected_on_long_rows():
+    """A column loop that ends at 4096 (the longest rows tested before) on a 9216-column row: the probabilities of
+    every column are normalised by the sum of the first 4096 only."""
+    g = torch.Generator().manual_seed(22)
+    s = torch.randn(8, 9216, generator=g)
+    assert bounds.softmax_check(softmax_restated(s, 0.5), s, 0.5).ok
+    rep = bounds.softmax_check(softmax_restated(s, 0.5, "stop_4096"), s, 0.5)
+    print(rep)
+    assert not rep.ok, str(rep)
 
 
 @pytest.mark.parametrize("mutant", ["round_p", "skip_stride"])

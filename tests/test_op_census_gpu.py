@@ -41,8 +41,11 @@ def _desc(t):
 class CheckedOps:
     """CudaOps with a float64 check after every call (records, never raises)."""
 
-    def __init__(self, inner):
+    def __init__(self, inner, max_elems=None):
+        """max_elems: bytes of one float64 intermediate of the GEMM, softmax and attention checks, which then run in row
+        chunks (bounds.gemm_check); None checks each GEMM and softmax call whole."""
         self.inner = inner
+        self.max_elems = max_elems
         self.ref = RefOps(DEV, compute_dtype=torch.float64)
         self.records = defaultdict(list)          # kind -> [(elementwise ratio, aggregate ratio)]
         self.failures = []
@@ -74,7 +77,7 @@ class CheckedOps:
             st = kw["stats_out"]
             if not torch.equal(st, bounds.stats_restated(out.reshape(M, No))):
                 self._fail(f"stats_out order: {what}")
-        rep = bounds.gemm_check(out, a0, w, splits=8, what=what, **snap)
+        rep = bounds.gemm_check(out, a0, w, splits=8, what=what, max_elems=self.max_elems, **snap)
         kind = "conv3x3" if kw.get("conv") is not None else "gemm+ln" if kw.get("ln") is not None else "gemm"
         self.records[kind + (" fp32" if out.dtype == torch.float32 else "")].append((rep.ratio, rep.agg_ratio))
         if not rep.ok:
@@ -84,7 +87,8 @@ class CheckedOps:
         q0, k0, v0 = q.clone(), k.clone(), v.clone()
         self.inner.attention(q, k, v, out, heads, d_head, causal=causal)
         torch.cuda.synchronize()
-        rep = bounds.attention_check(out, q0, k0, v0, heads, d_head, causal=causal,
+        chunk = {} if self.max_elems is None else dict(max_elems=self.max_elems)
+        rep = bounds.attention_check(out, q0, k0, v0, heads, d_head, causal=causal, **chunk,
                                      what=f"attention q={_desc(q)} k={_desc(k)} out={_desc(out)} heads={heads} d={d_head} causal={causal}")
         self.records["attention"].append((rep.ratio, 0.0))
         if not rep.ok:
@@ -129,7 +133,7 @@ class CheckedOps:
         s0 = s.clone()
         self.inner.softmax_rows(s, p, scale)
         torch.cuda.synchronize()
-        self._record("softmax_rows", bounds.softmax_check(p, s0, scale, what=f"softmax_rows s={_desc(s)}"))
+        self._record("softmax_rows", bounds.softmax_check(p, s0, scale, what=f"softmax_rows s={_desc(s)}", max_elems=self.max_elems))
 
     def conv_in(self, x, extra, w, bias, out):
         self.inner.conv_in(x, extra, w, bias, out)
