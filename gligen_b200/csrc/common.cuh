@@ -230,6 +230,14 @@ __device__ __forceinline__ float geglu_f(float x, float g) {
   const float h = 0.5f * g;
   return x * fmaf(h, erf_rational3(g * 0.70710678118654752f), h);
 }
+// Keys cubic convolution (A = -0.75, PyTorch's upsample_bicubic2d): weights of the taps at distance t + 1, t, 1 - t, 2 - t from
+// the source coordinate, t in [0, 1).  Shared by resize_plane (frontend.cu) and grid_resample_gate (fuser.cu).
+__device__ __forceinline__ float cubic1(float t, float A) { return ((A + 2.f) * t - (A + 3.f)) * t * t + 1.f; }
+__device__ __forceinline__ float cubic2(float t, float A) { return ((A * t - 5.f * A) * t + 8.f * A) * t - 4.f * A; }
+__device__ __forceinline__ void cubic_coeffs(float t, float* c) {
+  const float A = -0.75f;
+  c[0] = cubic2(t + 1.f, A); c[1] = cubic1(t, A); c[2] = cubic1(1.f - t, A); c[3] = cubic2(2.f - t, A);
+}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);

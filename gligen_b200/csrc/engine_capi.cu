@@ -117,6 +117,10 @@ int dispatch(const EOp& op, void* st) {
   if (n == "glg_conv2d_small")
     return glg_conv2d_small((const float*)A_P(0), (const float*)A_P(1), (const float*)A_P(2), (float*)A_P(3), A_I32(4), A_I32(5), A_I32(6), A_I32(7),
                             A_I32(8), A_I32(9), A_I32(10), A_I32(11), A_I32(12), A_I32(13), A_I32(14), st);
+  // gatedSA2 fuser: the resampled, gated residual of the grounding rows (per step)
+  if (n == "glg_grid_resample_gate")
+    return glg_grid_resample_gate((const float*)A_P(0), A_I(1), A_P(2), A_I(3), (const float*)A_P(4), (float*)A_P(5), A_I(6), A_I32(7), A_I32(8),
+                                  A_I32(9), A_I32(10), st);
   return set_error("glg_engine_run: unknown op '" + n + "' in the plan");
 }
 }  // namespace

@@ -201,13 +201,8 @@ __global__ void __launch_bounds__(256) dwconv7_ln_kernel(const bf16* __restrict_
   }
 }
 
-// ---- F.interpolate on NCHW fp32 planes: mode 0 nearest, 1 bicubic (align_corners=False, A = -0.75, border-clamped taps) ----
-__device__ __forceinline__ float cubic1(float t, float A) { return ((A + 2.f) * t - (A + 3.f)) * t * t + 1.f; }
-__device__ __forceinline__ float cubic2(float t, float A) { return ((A * t - 5.f * A) * t + 8.f * A) * t - 4.f * A; }
-__device__ __forceinline__ void cubic_coeffs(float t, float* c) {
-  const float A = -0.75f;
-  c[0] = cubic2(t + 1.f, A); c[1] = cubic1(t, A); c[2] = cubic1(1.f - t, A); c[3] = cubic2(2.f - t, A);
-}
+// ---- F.interpolate on NCHW fp32 planes: mode 0 nearest, 1 bicubic (align_corners=False, A = -0.75, border-clamped taps;
+// Keys coefficients in common.cuh) ----
 __global__ void resize_plane_kernel(const float* __restrict__ x, long long x_batch, float* __restrict__ y, int B, int C, int Hs, int Ws,
                                     int Ho, int Wo, int mode) {
   pdl_trigger();

@@ -10,10 +10,11 @@ restructurings, all exact in real arithmetic:
   * Q/K/V projections fused into one GEMM, GEGLU fused into the FF1 epilogue, bias / time-embedding /
     residual / tanh-gate adds fused into GEMM epilogues, the 22 ResBlock emb projections in one GEMM;
   * cond and uncond passes of classifier-free guidance can run as one 2B batch;
-  * the gated self-attention fuser is skipped when scale == 0 (x + 0*f(x), attention.py:241-242).
+  * the fuser (gatedSA, gatedCA or gatedSA2) is skipped when scale == 0 (x + 0*f(x), attention.py:241-242).
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Tuple
 
@@ -138,11 +139,30 @@ class Engine(EngineBase):
                     W[f"{p}.proj_out.w"], W[f"{p}.proj_out.b"] = self._a(sd[f"{p}.proj_out.weight"].reshape(C, C)), self._f(sd[f"{p}.proj_out.bias"])
                     tb = f"{p}.transformer_blocks.0"
                     # every LayerNorm -> Linear pair is folded (see include/gligen_b200.h "LayerNorm fold")
-                    for a, nrm in (("attn1", "norm1"), ("fuser.attn", "fuser.norm1")):
+                    fuser_ca = cfg.fuser_type == "gatedCA"
+                    fuser_sa = cfg.fuser_type == "gatedSA"
+                    for a, nrm in (("attn1", "norm1"),) + ((("fuser.attn", "fuser.norm1"),) if fuser_sa else ()):
                         wq = torch.cat([sd[f"{tb}.{a}.to_q.weight"], sd[f"{tb}.{a}.to_k.weight"], sd[f"{tb}.{a}.to_v.weight"]], dim=0)
                         wf, cs, b = self._fold_ln(wq, None, sd[f"{tb}.{nrm}.weight"], sd[f"{tb}.{nrm}.bias"])
                         W[f"{tb}.{a}.qkv.w"], W[f"{tb}.{a}.qkv.s"], W[f"{tb}.{a}.qkv.b"] = wf.to(self.dev).contiguous(), self._f(cs), self._f(b)
                         W[f"{tb}.{a}.out.w"], W[f"{tb}.{a}.out.b"] = self._a(sd[f"{tb}.{a}.to_out.0.weight"]), self._f(sd[f"{tb}.{a}.to_out.0.bias"])
+                    if cfg.fuser_type == "gatedSA2":
+                        # GatedSelfAttentionDense2 (attention.py:269-297): the grounding rows are the only queries, so Q (rows 0:C of the
+                        # norm1-folded QKV) and K/V (rows C:3C) are two GEMM weights: K/V for every row, Q for the grounding rows only
+                        fa = f"{tb}.fuser.attn"
+                        wq = torch.cat([sd[f"{fa}.to_q.weight"], sd[f"{fa}.to_k.weight"], sd[f"{fa}.to_v.weight"]], dim=0)
+                        wf, cs, b = self._fold_ln(wq, None, sd[f"{tb}.fuser.norm1.weight"], sd[f"{tb}.fuser.norm1.bias"])
+                        for part, rows in (("q", slice(0, C)), ("kv", slice(C, 3 * C))):      # each slot owns its storage (export)
+                            W[f"{fa}.{part}.w"] = wf[rows].clone().to(self.dev)
+                            W[f"{fa}.{part}.s"], W[f"{fa}.{part}.b"] = self._f(cs[rows].clone()), self._f(b[rows].clone())
+                        W[f"{fa}.out.w"], W[f"{fa}.out.b"] = self._a(sd[f"{fa}.to_out.0.weight"]), self._f(sd[f"{fa}.to_out.0.bias"])
+                    if fuser_ca:
+                        # GatedCrossAttentionDense (attention.py:190-212): norm1 folded into to_q like attn2's; K / V of the raw tokens
+                        fa = f"{tb}.fuser.attn"
+                        wf, cs, b = self._fold_ln(sd[f"{fa}.to_q.weight"], None, sd[f"{tb}.fuser.norm1.weight"], sd[f"{tb}.fuser.norm1.bias"])
+                        W[f"{fa}.q.w"], W[f"{fa}.q.s"], W[f"{fa}.q.b"] = wf.to(self.dev).contiguous(), self._f(cs), self._f(b)
+                        W[f"{fa}.kv.w"] = self._a(torch.cat([sd[f"{fa}.to_k.weight"], sd[f"{fa}.to_v.weight"]], dim=0))
+                        W[f"{fa}.out.w"], W[f"{fa}.out.b"] = self._a(sd[f"{fa}.to_out.0.weight"]), self._f(sd[f"{fa}.to_out.0.bias"])
                     wf, cs, b = self._fold_ln(sd[f"{tb}.attn2.to_q.weight"], None, sd[f"{tb}.norm2.weight"], sd[f"{tb}.norm2.bias"])
                     W[f"{tb}.attn2.q.w"], W[f"{tb}.attn2.q.s"], W[f"{tb}.attn2.q.b"] = wf.to(self.dev).contiguous(), self._f(cs), self._f(b)
                     W[f"{tb}.attn2.kv.w"] = self._a(torch.cat([sd[f"{tb}.attn2.to_k.weight"], sd[f"{tb}.attn2.to_v.weight"]], dim=0))
@@ -153,7 +173,8 @@ class Engine(EngineBase):
                         w1, s1, b1 = self._pack_geglu(wf, cs, b)
                         W[f"{tb}.{f}.w1"], W[f"{tb}.{f}.s1"], W[f"{tb}.{f}.b1"] = w1.to(self.dev).contiguous(), self._f(s1), self._f(b1)
                         W[f"{tb}.{f}.w2"], W[f"{tb}.{f}.b2"] = self._a(sd[f"{tb}.{f}.net.2.weight"]), self._f(sd[f"{tb}.{f}.net.2.bias"])
-                    W[f"{tb}.fuser.linear.w"], W[f"{tb}.fuser.linear.b"] = self._a(sd[f"{tb}.fuser.linear.weight"]), self._f(sd[f"{tb}.fuser.linear.bias"])
+                    if not fuser_ca:
+                        W[f"{tb}.fuser.linear.w"], W[f"{tb}.fuser.linear.b"] = self._a(sd[f"{tb}.fuser.linear.weight"]), self._f(sd[f"{tb}.fuser.linear.bias"])
         W["out.gn.g"], W["out.gn.b"] = self._f(sd["out.0.weight"]), self._f(sd["out.0.bias"])
         W["out.w"] = self._f(sd["out.2.weight"].permute(2, 3, 0, 1).reshape(9, cfg.out_channels, cfg.model_channels))
         W["out.b"] = self._f(sd["out.2.bias"])
@@ -412,6 +433,93 @@ class Engine(EngineBase):
                 res = x
             P.add(f"{p}.conv2", lambda: ops.gemm(a2, W[f"{p}.conv2.w"], out, bias=W[f"{p}.conv2.b"], residual=res, conv=(Bt, H, Wd)))
 
+        EPS = 1e-5
+
+        def emit_grounding_linear(fu, C, NS):
+            """gatedSA / gatedSA2: objs' = linear(objs) with the LayerNorm partials of its rows, once per sample (static)."""
+            objp = self._buf(S * Bt * N * C).view(S, Bt * N, C)
+            ostat = self._buf(S * Bt * N * NS * 2, f32).view(NS, S * Bt * N, 2)     # slot-major over all streams' rows
+            return objp, ostat
+
+        def emit_grounding_qkv(fu, T, C, NS):
+            """gatedSA: objs' = linear(objs) and the grounding rows of LN(cat[x, objs']) @ Wqkv, once per sample (static),
+            into rows [T, T+G) of a per-layer [Bt, T+G, 3C] buffer whose visual rows are written every step."""
+            objp, ostat = emit_grounding_linear(fu, C, NS)
+            qkv2 = self._buf(Bt * (T + G) * 3 * C).view(Bt, T + G, 3 * C)
+            P.add(f"{fu}.linear", lambda: ops.gemm(objs.view(S * Bt * N, D), W[f"{fu}.linear.w"], objp.view(S * Bt * N, C),
+                                                  bias=W[f"{fu}.linear.b"], stats_out=ostat), fuser=True, static=True)
+            for si in range(S):
+                P.add(f"{fu}.attn.qkv.objs{si}", lambda si=si: ops.gemm(
+                    objp[si], W[f"{fu}.attn.qkv.w"], qkv2[:, T + si * N: T + (si + 1) * N], bias=W[f"{fu}.attn.qkv.b"],
+                    ln=(ostat[:, si * Bt * N: (si + 1) * Bt * N], W[f"{fu}.attn.qkv.s"], EPS)), fuser=True, static=True)
+            return qkv2
+
+        def emit_fuser_ff(fu, gi, xs, xst, ffh):
+            """x += scale*tanh(alpha_dense) * ff(norm2(x)), the second half of every fuser; norm2 folded into ff.1 on the
+            partials of the rows the gated attention residual just stored."""
+            P.add(f"{fu}.ff.1", lambda: ops.gemm(xs, W[f"{fu}.ff.w1"], ffh, bias=W[f"{fu}.ff.b1"], geglu=True,
+                                                ln=(xst, W[f"{fu}.ff.s1"], EPS)), fuser=True)
+            P.add(f"{fu}.ff.2", lambda: ops.gemm(ffh, W[f"{fu}.ff.w2"], xs, bias=W[f"{fu}.ff.b2"], gate=W["gates"][gi, 1:2],
+                                                residual=xs, stats_out=xst), fuser=True)
+
+        def emit_fuser_sa(tb, T, C, heads, d, gi, xs, xst, ao, ffh):
+            # -- fuser: GatedSelfAttentionDense (attention.py:236-244); skipped when scale == 0.
+            #    LN(cat[x, objs']) @ Wqkv is computed as two GEMMs into one per-layer [Bt, T+G, 3C] buffer: the
+            #    visual rows every step, the grounding rows (objs' = linear(objs) is timestep-invariant) once.
+            fu = f"{tb}.fuser"
+            qkv2 = emit_grounding_qkv(fu, T, C, C // 32)
+            P.add(f"{fu}.attn.qkv", lambda: ops.gemm(xs, W[f"{fu}.attn.qkv.w"], qkv2[:, :T], bias=W[f"{fu}.attn.qkv.b"],
+                                                    ln=(xst, W[f"{fu}.attn.qkv.s"], EPS)), fuser=True)
+            P.add(f"{fu}.attn.core", lambda: ops.attention(qkv2[:, :T, :C], qkv2[:, :, C:2 * C], qkv2[:, :, 2 * C:], ao, heads, d), fuser=True)
+            P.add(f"{fu}.attn.out", lambda: ops.gemm(ao, W[f"{fu}.attn.out.w"], xs, bias=W[f"{fu}.attn.out.b"],
+                                                    gate=W["gates"][gi, 0:1], residual=xs, stats_out=xst), fuser=True)
+            emit_fuser_ff(fu, gi, xs, xst, ffh)
+
+        def emit_fuser_ca(tb, T, C, heads, d, gi, xs, xst, t0, ffh):
+            # -- fuser: GatedCrossAttentionDense (attention.py:207-212); skipped when scale == 0.  Queries from LN(x) (norm1 folded
+            #    into to_q), keys / values from the raw grounding tokens: timestep-invariant, projected once per sample into a
+            #    per-layer [Bt, G, 2C] buffer (one GEMM per grounding stream, streams in PositionNet order).
+            fu = f"{tb}.fuser"
+            kvc = self._buf(Bt * G * 2 * C).view(Bt, G, 2 * C)
+            q = view("ao", Bt, T, C)
+            for si in range(S):
+                P.add(f"{fu}.attn.kv.objs{si}", lambda si=si: ops.gemm(objs[si], W[f"{fu}.attn.kv.w"], kvc[:, si * N: (si + 1) * N]),
+                      fuser=True, static=True)
+            P.add(f"{fu}.attn.q", lambda: ops.gemm(xs, W[f"{fu}.attn.q.w"], q, bias=W[f"{fu}.attn.q.b"], ln=(xst, W[f"{fu}.attn.q.s"], EPS)),
+                  fuser=True)
+            P.add(f"{fu}.attn.core", lambda: ops.attention(q, kvc[:, :, :C], kvc[:, :, C:], t0, heads, d), fuser=True)
+            P.add(f"{fu}.attn.out", lambda: ops.gemm(t0, W[f"{fu}.attn.out.w"], xs, bias=W[f"{fu}.attn.out.b"],
+                                                    gate=W["gates"][gi, 0:1], residual=xs, stats_out=xst), fuser=True)
+            emit_fuser_ff(fu, gi, xs, xst, ffh)
+
+        def emit_fuser_sa2(tb, T, C, heads, d, gi, xs, xst, ffh, H, Wd):
+            # -- fuser: GatedSelfAttentionDense2 (attention.py:269-297); skipped when scale == 0.  Only the G grounding rows of the
+            #    self-attention over LN(cat[x, objs']) are kept, so they are the only queries and the visual rows only need K / V.
+            #    Their to_out rows (fp32) are the g x g grid that glg_grid_resample_gate resamples onto the n x n visual grid and
+            #    adds, gated, to x - with the LayerNorm partials that ff.1 folds.
+            fu = f"{tb}.fuser"
+            g = math.isqrt(G)
+            objp, ostat = emit_grounding_linear(fu, C, C // 32)
+            qg = self._buf(Bt * G * C).view(Bt, G, C)                        # queries: the grounding rows only (static)
+            kv2 = self._buf(Bt * (T + G) * 2 * C).view(Bt, T + G, 2 * C)     # K/V: visual rows every step, grounding rows static
+            og = self._buf(Bt * G * C).view(Bt, G, C)                        # attention output of the grounding rows
+            res = self._buf(Bt * G * C, f32).view(Bt, G, C)                  # their to_out projection: the grid to resample
+            P.add(f"{fu}.linear", lambda: ops.gemm(objs.view(S * Bt * N, D), W[f"{fu}.linear.w"], objp.view(S * Bt * N, C),
+                                                  bias=W[f"{fu}.linear.b"], stats_out=ostat), fuser=True, static=True)
+            for si in range(S):
+                ln = lambda part, si=si: (ostat[:, si * Bt * N: (si + 1) * Bt * N], W[f"{fu}.attn.{part}.s"], EPS)
+                P.add(f"{fu}.attn.q.objs{si}", lambda si=si, ln=ln: ops.gemm(
+                    objp[si], W[f"{fu}.attn.q.w"], qg[:, si * N: (si + 1) * N], bias=W[f"{fu}.attn.q.b"], ln=ln("q")), fuser=True, static=True)
+                P.add(f"{fu}.attn.kv.objs{si}", lambda si=si, ln=ln: ops.gemm(
+                    objp[si], W[f"{fu}.attn.kv.w"], kv2[:, T + si * N: T + (si + 1) * N], bias=W[f"{fu}.attn.kv.b"], ln=ln("kv")),
+                      fuser=True, static=True)
+            P.add(f"{fu}.attn.kv", lambda: ops.gemm(xs, W[f"{fu}.attn.kv.w"], kv2[:, :T], bias=W[f"{fu}.attn.kv.b"],
+                                                   ln=(xst, W[f"{fu}.attn.kv.s"], EPS)), fuser=True)
+            P.add(f"{fu}.attn.core", lambda: ops.attention(qg, kv2[:, :, :C], kv2[:, :, C:], og, heads, d), fuser=True)
+            P.add(f"{fu}.attn.out", lambda: ops.gemm(og, W[f"{fu}.attn.out.w"], res, bias=W[f"{fu}.attn.out.b"]), fuser=True)
+            P.add(f"{fu}.resample", lambda: ops.grid_resample_gate(res, xs, W["gates"][gi, 0:1], xst, g, H), fuser=True)
+            emit_fuser_ff(fu, gi, xs, xst, ffh)
+
         def emit_st(ly, x_in, out, H, Wd):
             p, T, C = ly.prefix, H * Wd, ly.cin
             tb = f"{p}.transformer_blocks.0"
@@ -424,7 +532,6 @@ class Engine(EngineBase):
             ffh = view("ffh", Bt, T, 4 * C)
             qkv = view("qkv", Bt, T, 3 * C)
             xst = view("xstat", NS, Bt * T, 2)             # slot-major (sum, sumsq) partials of the CURRENT xs rows
-            EPS = 1e-5
             P.add(f"{p}.gn", lambda: ops.groupnorm(x_in, t0, W[f"{p}.gn.g"], W[f"{p}.gn.b"], stats, 32, 1e-6, False))
             P.add(f"{p}.proj_in", lambda: ops.gemm(t0, W[f"{p}.proj_in.w"], xs, bias=W[f"{p}.proj_in.b"], stats_out=xst))
             # -- attn1 (attention.py:334); norm1 folded into the QKV GEMM
@@ -432,28 +539,12 @@ class Engine(EngineBase):
                                                       ln=(xst, W[f"{tb}.attn1.qkv.s"], EPS)))
             P.add(f"{tb}.attn1.core", lambda: ops.attention(qkv[:, :, :C], qkv[:, :, C:2 * C], qkv[:, :, 2 * C:], ao, heads, d))
             P.add(f"{tb}.attn1.out", lambda: ops.gemm(ao, W[f"{tb}.attn1.out.w"], xs, bias=W[f"{tb}.attn1.out.b"], residual=xs, stats_out=xst))
-            # -- fuser: GatedSelfAttentionDense (attention.py:236-244); skipped when scale == 0.
-            #    LN(cat[x, objs']) @ Wqkv is computed as two GEMMs into one per-layer [Bt, T+G, 3C] buffer: the
-            #    visual rows every step, the grounding rows (objs' = linear(objs) is timestep-invariant) once.
-            fu = f"{tb}.fuser"
-            objp = self._buf(S * Bt * N * C).view(S, Bt * N, C)
-            ostat = self._buf(S * Bt * N * NS * 2, f32).view(NS, S * Bt * N, 2)     # slot-major over all streams' rows
-            qkv2 = self._buf(Bt * (T + G) * 3 * C).view(Bt, T + G, 3 * C)
-            P.add(f"{fu}.linear", lambda: ops.gemm(objs.view(S * Bt * N, D), W[f"{fu}.linear.w"], objp.view(S * Bt * N, C),
-                                                  bias=W[f"{fu}.linear.b"], stats_out=ostat), fuser=True, static=True)
-            for si in range(S):
-                P.add(f"{fu}.attn.qkv.objs{si}", lambda si=si: ops.gemm(
-                    objp[si], W[f"{fu}.attn.qkv.w"], qkv2[:, T + si * N: T + (si + 1) * N], bias=W[f"{fu}.attn.qkv.b"],
-                    ln=(ostat[:, si * Bt * N: (si + 1) * Bt * N], W[f"{fu}.attn.qkv.s"], EPS)), fuser=True, static=True)
-            P.add(f"{fu}.attn.qkv", lambda: ops.gemm(xs, W[f"{fu}.attn.qkv.w"], qkv2[:, :T], bias=W[f"{fu}.attn.qkv.b"],
-                                                    ln=(xst, W[f"{fu}.attn.qkv.s"], EPS)), fuser=True)
-            P.add(f"{fu}.attn.core", lambda: ops.attention(qkv2[:, :T, :C], qkv2[:, :, C:2 * C], qkv2[:, :, 2 * C:], ao, heads, d), fuser=True)
-            P.add(f"{fu}.attn.out", lambda: ops.gemm(ao, W[f"{fu}.attn.out.w"], xs, bias=W[f"{fu}.attn.out.b"],
-                                                    gate=W["gates"][gi, 0:1], residual=xs, stats_out=xst), fuser=True)
-            P.add(f"{fu}.ff.1", lambda: ops.gemm(xs, W[f"{fu}.ff.w1"], ffh, bias=W[f"{fu}.ff.b1"], geglu=True,
-                                                ln=(xst, W[f"{fu}.ff.s1"], EPS)), fuser=True)
-            P.add(f"{fu}.ff.2", lambda: ops.gemm(ffh, W[f"{fu}.ff.w2"], xs, bias=W[f"{fu}.ff.b2"], gate=W["gates"][gi, 1:2],
-                                                residual=xs, stats_out=xst), fuser=True)
+            if cfg.fuser_type == "gatedCA":
+                emit_fuser_ca(tb, T, C, heads, d, gi, xs, xst, t0, ffh)
+            elif cfg.fuser_type == "gatedSA2":
+                emit_fuser_sa2(tb, T, C, heads, d, gi, xs, xst, ffh, H, Wd)
+            else:
+                emit_fuser_sa(tb, T, C, heads, d, gi, xs, xst, ao, ffh)
             # -- attn2: cross attention to the text context (attention.py:336); K/V of the context are static
             q = view("ao", Bt, T, C)            # ao is free between attention calls: reuse as Q, write O to t0
             kv = self._buf(Bt * nctx * 2 * C).view(Bt, nctx, 2 * C)  # per layer: static across timesteps
@@ -519,6 +610,9 @@ class Engine(EngineBase):
         H = self.cfg.image_size if H is None else H
         W = self.cfg.image_size if W is None else W
         self.check_latent_size(H, W)
+        G = N * self.n_streams
+        if self.cfg.fuser_type == "gatedSA2" and math.isqrt(G) ** 2 != G:
+            raise AssertionError("Grounding tokens must be square rootable")     # the reference's assert (attention.py:278)
         # one plan (and static-part cache) per latent size and batch chunk; the square default size keeps the short key
         size = () if H == W == self.cfg.image_size else (H, W)
         key = (Bt, N, nctx) + size + ((slot,) if slot else ())
@@ -535,6 +629,11 @@ class Engine(EngineBase):
         f = max(blk.ds for blk in self.blocks)
         if H <= 0 or W <= 0 or H % f or W % f:
             raise ValueError(f"latent {H}x{W}: both sides must be positive multiples of {f} (one per stride-2 downsample)")
+        if self.cfg.fuser_type == "gatedSA2" and H != W:
+            # the reference only asserts that H*W is a perfect square (attention.py:277) and would resample the grounding rows onto a
+            # sqrt(H*W)-sided square that is not the latent's geometry: refused here
+            raise ValueError(f"latent {H}x{W}: gatedSA2 fusers resample the grounding tokens onto a square visual grid, so the latent "
+                             f"must be square")
         n = self.cfg.image_size
         if self.cfg.ds_out_dim and (H, W) != (n, n):
             raise ValueError(f"latent {H}x{W}: the grounding downsampler of {self.cfg.tokenizer} models writes {n}x{n} planes that "

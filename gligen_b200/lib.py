@@ -73,6 +73,7 @@ SIGNATURES = {
     "glg_spatial_tokens": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p]),
     "glg_resize_plane": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "glg_conv2d_small": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "glg_grid_resample_gate": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
     "glg_engine_load": (c_int, [C.c_char_p, C.POINTER(c_void_p)]),
     "glg_engine_buffer": (c_int, [c_void_p, C.c_char_p, C.POINTER(c_void_p), C.POINTER(c_int64)]),
     "glg_engine_write": (c_int, [c_void_p, C.c_char_p, c_void_p, c_int64, c_void_p]),

@@ -338,6 +338,22 @@ class CudaOps:
                                           {"nearest": 0, "bicubic": 1}[mode], self._stream()), "glg_resize_plane")
         self._note("resize_plane")
 
+    # -- gatedSA2 fuser ------------------------------------------------------------------------------------------------------
+    def grid_resample_gate(self, grid, x, gate, stats_out, g: int, n: int):
+        """x [B, n*n, C] bf16 rows += gate * bicubic_{g->n}(grid) in place; grid fp32 [B, g*g, C] (row-major tokens, any batch
+        stride); gate a device fp32 scalar; stats_out [C/32, B*n*n, 2] fp32 slot-major (may be a row range of a larger buffer):
+        the LayerNorm partials of the stored rows, as gemm(stats_out=...)."""
+        B, GG, Cc = grid.shape
+        assert grid.dtype == torch.float32 and grid.stride(2) == 1 and grid.stride(1) == Cc and GG == g * g, (grid.shape, grid.stride(), g)
+        xp, rows, Cx, ldx = _rows_view(x)
+        assert rows == B * n * n and Cx == Cc, (x.shape, B, n, Cc)
+        so = stats_out
+        assert so.dtype == torch.float32 and so.dim() == 3 and so.shape == (Cc // 32, rows, 2) and so.stride(2) == 1 and so.stride(1) == 2
+        assert gate.dtype == torch.float32 and gate.numel() == 1
+        L.check(self._c.glg_grid_resample_gate(grid.data_ptr(), grid.stride(0), xp, ldx, gate.data_ptr(), so.data_ptr(), so.stride(0) // 2,
+                                                B, g, n, Cc, self._stream()), "glg_grid_resample_gate")
+        self._note("grid_resample_gate", 0.0, 4.0 * rows * Cc + 8.0 * rows * (Cc // 32))
+
     def conv2d_small(self, x, w, bias, y, k: int, stride: int, pad: int, silu: bool, virtual=None):
         """Direct Conv2d on fp32 NCHW, Cout in {3, 4, 8, 16}; w fp32 packed [Cin*k*k, Cout]; `virtual=(Hv, Wv)`: the input is x
         resampled (nearest) onto that grid first."""

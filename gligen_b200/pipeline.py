@@ -58,7 +58,7 @@ def model_config(cfg: UNetConfig) -> Dict:
     return dict(target="ldm.modules.diffusionmodules.openaimodel.UNetModel", params=dict(**extra, **dict(
         image_size=cfg.image_size, in_channels=cfg.in_channels, out_channels=cfg.out_channels, model_channels=cfg.model_channels,
         attention_resolutions=list(cfg.attention_resolutions), num_res_blocks=cfg.num_res_blocks, channel_mult=list(cfg.channel_mult),
-        num_heads=cfg.num_heads, transformer_depth=1, context_dim=cfg.context_dim, fuser_type="gatedSA", use_checkpoint=True,
+        num_heads=cfg.num_heads, transformer_depth=1, context_dim=cfg.context_dim, fuser_type=cfg.fuser_type, use_checkpoint=True,
         inpaint_mode=cfg.inpaint_mode, grounding_tokenizer=dict(target=tgt, params=par(cfg)))))
 
 

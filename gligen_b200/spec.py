@@ -28,6 +28,8 @@ class UNetConfig:
     num_heads: int = 8
     transformer_depth: int = 1
     context_dim: int = 768
+    # "gatedSA" (every shipped config), "gatedCA" (cross-attention to the grounding tokens) or "gatedSA2" (self-attention whose
+    # grounding rows are resampled onto the visual grid), reference attention.py:190-297
     fuser_type: str = "gatedSA"
     inpaint_mode: bool = False
     # grounding tokenizer: "text" | "text_image" | "keypoint" (discrete objects) or one of SPATIAL_TOKENIZERS
@@ -112,6 +114,19 @@ TINY_CANNY = replace(TINY, tokenizer="canny", ds_out_dim=8, tok_resize=128, ds_r
 TINY_DEPTH = replace(TINY, tokenizer="depth", ds_out_dim=8, tok_resize=128, ds_resize=64)
 TINY_NORMAL = replace(TINY, tokenizer="normal", ds_out_dim=8, tok_resize=128, ds_resize=64)
 TINY_SEM = replace(TINY, tokenizer="sem", ds_out_dim=8, tok_resize=128, ds_resize=64, sem_in_dim=24)
+# the other two fusers the reference builds (BasicTransformerBlock, attention.py:313-321).  gatedCA: any token count (keypoint with
+# 8 persons = 136 tokens takes the long-key attention kernel); gatedSA2 needs a square token count: the spatial tokenizers' 16 / 64
+SD14_BOX_TEXT_GATED_CA = replace(SD14_BOX_TEXT, fuser_type="gatedCA")
+SD14_HED_GATED_SA2 = replace(SD14_HED, fuser_type="gatedSA2")
+TINY_GATED_CA = replace(TINY, fuser_type="gatedCA")
+TINY_TEXT_IMAGE_GATED_CA = replace(TINY_TEXT_IMAGE, fuser_type="gatedCA")
+TINY_KEYPOINT_GATED_CA = replace(TINY_KEYPOINT, fuser_type="gatedCA", max_persons=8)
+TINY_HED_GATED_SA2 = replace(TINY_HED, fuser_type="gatedSA2")
+FUSER_TYPES = ("gatedSA", "gatedCA", "gatedSA2")
+# small 320-channel models for scheduled-sampling loops: the reference's restore_first_conv_from_SD builds SD's 4 -> 320 first conv
+# whatever the model (openaimodel.py:400-413), so a loop with alpha = 0 steps needs model_channels = 320.  Not in NAMED_CONFIGS.
+SAMPLING_GATED_CA = replace(TINY_GATED_CA, model_channels=320, channel_mult=(1, 1), num_res_blocks=1, attention_resolutions=(1, 2))
+SAMPLING_HED_GATED_SA2 = replace(TINY_HED_GATED_SA2, model_channels=320, channel_mult=(1, 1, 1), num_res_blocks=1, attention_resolutions=(2, 4))
 
 NAMED_CONFIGS = {
     "sd14_box_text": SD14_BOX_TEXT,
@@ -124,6 +139,9 @@ NAMED_CONFIGS = {
     "tiny_inpaint": TINY_INPAINT,
     "sd14_hed": SD14_HED, "sd14_canny": SD14_CANNY, "sd14_depth": SD14_DEPTH, "sd14_normal": SD14_NORMAL, "sd14_sem": SD14_SEM,
     "tiny_hed": TINY_HED, "tiny_canny": TINY_CANNY, "tiny_depth": TINY_DEPTH, "tiny_normal": TINY_NORMAL, "tiny_sem": TINY_SEM,
+    "sd14_box_text_gated_ca": SD14_BOX_TEXT_GATED_CA, "sd14_hed_gated_sa2": SD14_HED_GATED_SA2,
+    "tiny_gated_ca": TINY_GATED_CA, "tiny_text_image_gated_ca": TINY_TEXT_IMAGE_GATED_CA, "tiny_keypoint_gated_ca": TINY_KEYPOINT_GATED_CA,
+    "tiny_hed_gated_sa2": TINY_HED_GATED_SA2,
 }
 
 
@@ -272,9 +290,12 @@ def unet_param_shapes(cfg: UNetConfig) -> "OrderedDict[str, tuple]":
             fu = f"{tb}.fuser"
             p[f"{fu}.alpha_attn"] = ()
             p[f"{fu}.alpha_dense"] = ()
-            p[f"{fu}.linear.weight"] = (c, cfg.context_dim)
-            p[f"{fu}.linear.bias"] = (c,)
-            _attn_params(p, f"{fu}.attn", c, c)
+            if cfg.fuser_type == "gatedCA":          # GatedCrossAttentionDense: no linear, K / V project the tokens themselves
+                _attn_params(p, f"{fu}.attn", c, cfg.context_dim)
+            else:                                     # GatedSelfAttentionDense / GatedSelfAttentionDense2: the same parameters
+                p[f"{fu}.linear.weight"] = (c, cfg.context_dim)
+                p[f"{fu}.linear.bias"] = (c,)
+                _attn_params(p, f"{fu}.attn", c, c)
             _ff_params(p, f"{fu}.ff", c)
             _norm_params(p, f"{fu}.norm1", c)
             _norm_params(p, f"{fu}.norm2", c)
@@ -419,7 +440,11 @@ def flops_per_forward(cfg: UNetConfig, G: int, fuser_on: bool = True, latent: Op
                 C, T = ly.cin, hw
                 total += 4.0 * T * C * C                                   # proj in/out
                 total += 8.0 * T * C * C + 4.0 * T * T * C                 # attn1
-                if fuser_on:
+                if fuser_on and cfg.fuser_type == "gatedCA":          # q, K/V of the tokens, attention T x G, out, ff
+                    total += 4.0 * T * C * C + 4.0 * G * ctx * C + 4.0 * T * G * C + 24.0 * T * C * C
+                elif fuser_on and cfg.fuser_type == "gatedSA2":       # only the G grounding rows query and leave the attention
+                    total += 2.0 * G * ctx * C + 6.0 * G * C * C + 4.0 * T * C * C + 4.0 * G * (T + G) * C + 2.0 * G * C * C + 24.0 * T * C * C
+                elif fuser_on:
                     total += 2.0 * G * ctx * C + 8.0 * (T + G) * C * C + 4.0 * (T + G) ** 2 * C + 24.0 * T * C * C
                 total += 4.0 * T * C * C + 4.0 * 77 * ctx * C + 4.0 * T * 77 * C   # attn2
                 total += 24.0 * T * C * C                                  # ff

@@ -227,6 +227,18 @@ int glg_resize_plane(const float* x, int64_t x_batch_stride, float* y, int32_t B
 int glg_conv2d_small(const float* x, const float* w, const float* bias, float* y, int32_t B, int32_t Cin, int32_t Hs, int32_t Ws, int32_t Hv,
                      int32_t Wv, int32_t Cout, int32_t k, int32_t stride, int32_t pad, int32_t silu, void* stream);
 
+/* ---- gatedSA2 fuser residual (attention.py:283-291: the grounding rows of the fuser's self-attention, reshaped to a g x g
+ * grid, F.interpolate(mode='bicubic') onto the n x n visual grid, then the gated add x + scale*tanh(alpha_attn)*residual) ------
+ *   x[b, y*n + x', c] = bf16( x[b, y*n + x', c] + gate[0] * bicubic_{g->n}(grid[b])[y, x', c] )      in place
+ * grid fp32 [B][g*g][C] (row-major tokens, batch stride grid_batch_stride elements, 16-byte aligned); x bf16 rows b*n*n + p of
+ * stride ldx (>= C, multiple of 8, 16-byte aligned); gate a device fp32 scalar (scale * tanh(alpha_attn)).  Bicubic as
+ * glg_resize_plane: align_corners = False, A = -0.75, border-clamped taps (n < g is an unfiltered downsample, n == g the identity).
+ * stats_out SLOT-major [C/32][stats_slot_stride rows][2]: per (row, 32-column slot) the sum and sum of squares of the stored
+ * bf16 values - the stats_out contract of glg_gemm, so the norm2-folded FF GEMM that follows reads them as ln_stats.
+ * C a multiple of 32, g <= 19. */
+int glg_grid_resample_gate(const float* grid, int64_t grid_batch_stride, void* x, int64_t ldx, const float* gate, float* stats_out,
+                           int64_t stats_slot_stride, int32_t B, int32_t g, int32_t n, int32_t C, void* stream);
+
 /* ---- sampler update (plms.py:121-158, ddim.py:113-134), one fused fp32 kernel ---------------
  * e      = e_u + g*(e_c - e_u)                       (if e_uncond != NULL, else e = e_cond)
  * e'     = c0*e + c1*old1 + c2*old2 + c3*old3        (Adams-Bashforth / identity / improved Euler)

@@ -2,7 +2,8 @@
 
 In this engine these classes are parameter containers only: the arithmetic of
 reference ldm/modules/attention.py (SelfAttention :154-186, CrossAttention :102-149,
-GatedSelfAttentionDense :215-244, BasicTransformerBlock :303-338, SpatialTransformer :341-376) runs as
+GatedCrossAttentionDense :190-212, GatedSelfAttentionDense :215-244, GatedSelfAttentionDense2 :251-297, BasicTransformerBlock
+:303-338, SpatialTransformer :341-376) runs as
 fused sm_90a kernels driven by gligen_b200.engine; the containers exist so that
   * state_dict() keys equal the reference's (checkpoints load verbatim), and
   * `set_alpha_scale` (gligen_inference.py:24-28), which walks model.modules() and tests
@@ -87,7 +88,8 @@ class GatedSelfAttentionDense(ParamNode):
 
 
 class GatedCrossAttentionDense(ParamNode):
-    """Importable for `set_alpha_scale`; no shipped config selects fuser_type=gatedCA (not accelerated)."""
+    """fuser_type="gatedCA": gated cross-attention from the visual tokens to the grounding tokens, then the gated FF.  `scale`
+    as GatedSelfAttentionDense (set_alpha_scale matches this type too)."""
 
     def __init__(self):
         super().__init__()
@@ -95,7 +97,9 @@ class GatedCrossAttentionDense(ParamNode):
 
 
 class GatedSelfAttentionDense2(ParamNode):
-    """Importable name only; no shipped config selects fuser_type=gatedSA2 (not accelerated)."""
+    """fuser_type="gatedSA2": self-attention over [visual; grounding] tokens whose grounding rows, resampled (bicubic) from
+    their sqrt(G) x sqrt(G) grid onto the visual grid, are the gated residual.  `set_alpha_scale` does not match this type, so
+    scheduled sampling leaves it at scale 1, as in the reference; a `.scale` set by hand is honoured."""
 
     def __init__(self):
         super().__init__()

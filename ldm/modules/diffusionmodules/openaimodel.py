@@ -15,8 +15,8 @@ import torch
 import torch.nn as nn
 
 from gligen_b200.spec import UNetConfig, unet_param_shapes
-from ldm.modules.attention import (BasicTransformerBlock, CrossAttention, FeedForward, GatedSelfAttentionDense,
-                                   ParamNode, SelfAttention, SpatialTransformer, attach_params)
+from ldm.modules.attention import (BasicTransformerBlock, CrossAttention, FeedForward, GatedCrossAttentionDense, GatedSelfAttentionDense,
+                                   GatedSelfAttentionDense2, ParamNode, SelfAttention, SpatialTransformer, attach_params)
 from gligen_b200.spec import SPATIAL_TOKENIZERS
 from ldm.modules.diffusionmodules.grounding_common import downsampler_config, tokenizer_config
 from ldm.util import instantiate_from_config
@@ -46,13 +46,18 @@ class Upsample(ParamNode):
     pass
 
 
-def _node_class(path: str):
+_FUSER_CLASS = {"gatedSA": GatedSelfAttentionDense, "gatedCA": GatedCrossAttentionDense, "gatedSA2": GatedSelfAttentionDense2}
+
+
+def _node_class(path: str, fuser_type: str = "gatedSA"):
     """Container type for a module path (purely cosmetic except for the fuser, which set_alpha_scale finds by type)."""
     if re.fullmatch(r"(input_blocks|output_blocks)\.\d+|middle_block", path):
         return TimestepEmbedSequential
     if path.endswith(".fuser"):
-        return GatedSelfAttentionDense
-    if path.endswith((".attn1", ".fuser.attn")):
+        return _FUSER_CLASS[fuser_type]
+    if path.endswith(".fuser.attn"):
+        return CrossAttention if fuser_type == "gatedCA" else SelfAttention
+    if path.endswith(".attn1"):
         return SelfAttention
     if path.endswith(".attn2"):
         return CrossAttention
@@ -71,8 +76,6 @@ class UNetModel(ParamNode):
         super().__init__()
         assert fuser_type in ["gatedSA", "gatedSA2", "gatedCA"]
         unsupported = []
-        if fuser_type != "gatedSA":
-            unsupported.append(f"fuser_type={fuser_type} (every shipped config uses gatedSA)")
         target = (grounding_tokenizer or {}).get("target")
         ds_target = (grounding_downsampler or {}).get("target")
         if grounding_downsampler is not None and (ds_target not in _DOWNSAMPLERS or _DOWNSAMPLERS[ds_target] != _TOKENIZERS.get(target)):
@@ -119,9 +122,9 @@ class UNetModel(ParamNode):
             self.first_conv_type = "GLIGEN"
         shapes = unet_param_shapes(self.cfg)
         body = {k: v for k, v in shapes.items() if not k.startswith(("position_net.", "downsample_net."))}
-        attach_params(self, body, "", _node_class)
+        attach_params(self, body, "", lambda path: _node_class(path, fuser_type))
         self.position_net = instantiate_from_config(grounding_tokenizer)
-        self._fusers = [m for m in self.modules() if type(m) == GatedSelfAttentionDense]
+        self._fusers = [m for m in self.modules() if type(m) == _FUSER_CLASS[fuser_type]]
         self._engine = None
         self._engine_stale = True
         self._sd_conv_cache = None
