@@ -5,7 +5,7 @@ synchronises and checks the output against RefOps(float64) on the snapshot - the
 rounding-level bounds of tests/bounds.py, GroupNorm, the LayerNorms, softmax_rows and the edge convolutions with
 the bounds derived for them there, as are the embeddings, token rows, dwconv7_ln, the CLIP vision embed / head, the
 sampler update, and the resampling ops of the spatial modalities (resize_plane, conv2d_small) with the bounds of
-tests/bounds_resample.py; stats_out bit for bit
+tests/bounds_resample.py, the gatedSA2 grid_resample_gate with that of tests/fuser_checks.py; stats_out bit for bit
 against its documented summation order; cast, the copies and the patch gathers exactly.  The forwards run with seeded synthetic weights and no CUDA graphs, so
 every call of the plan is seen.  A failure lists every violating call with its shapes, strides, flags and tile choice."""
 import ctypes as C
@@ -18,6 +18,7 @@ import torch
 import bounds
 import bounds_resample
 from conftest import assert_close
+from fuser_checks import resample_gate_check, stats_check
 from ref_ops import RefOps
 
 pytestmark = pytest.mark.gpu
@@ -204,7 +205,28 @@ class CheckedOps:
         self.inner.conv2d_small(x, w, bias, y, k, stride, pad, silu, virtual=virtual)
         torch.cuda.synchronize()
         what = f"conv2d_small x={_desc(x)} y={_desc(y)} k={k} stride={stride} pad={pad} silu={silu} virtual={virtual}"
-        self._record("conv2d_small", bounds_resample.conv2d_small_check(y, x0, w, bias, k, stride, pad, silu, virtual, what=what))
+        # with max_elems, one image at a time (the float64 check holds every tap of the batch at once)
+        step = x.shape[0] if self.max_elems is None else 1
+        reps = [bounds_resample.conv2d_small_check(y[b:b + step], x0[b:b + step], w, bias, k, stride, pad, silu, virtual, what=f"{what} b={b}")
+                for b in range(0, x.shape[0], step)]
+        self._record("conv2d_small", max(reps, key=lambda r: (r.ratio, r.agg_ratio)))
+
+    def grid_resample_gate(self, grid, x, gate, stats_out, g, n):
+        x0, grid0 = x.clone(), grid.clone()
+        self.inner.grid_resample_gate(grid, x, gate, stats_out, g, n)
+        torch.cuda.synchronize()
+        B, C = grid.shape[0], grid.shape[2]
+        gv = float(gate.item())
+        worst = 0.0
+        for b in range(B):                              # one image at a time keeps the float64 gather small
+            rep = resample_gate_check(x[b:b + 1], x0[b:b + 1], grid0[b:b + 1], gv, g, n, what=f"grid_resample_gate g={g} n={n} C={C} b={b}")
+            worst = max(worst, rep.ratio)
+            if not rep.ok:
+                self._fail(str(rep))
+        rep = stats_check(stats_out, x.reshape(-1, C))
+        if not rep.ok:
+            self._fail(str(rep))
+        self.records["grid_resample_gate"].append((worst, 0.0))
 
     def _small(self, name, fn, *a, **kw):
         outs, rel, max_rel = SMALL_OPS[name]
