@@ -345,6 +345,51 @@ __global__ void sampler_update_kernel(const float* __restrict__ x, const float* 
   }
 }
 
+// One DPM-Solver++ multistep update (include/gligen_b200.h, glg_dpm_update).  Elements [0, 4 n4) move as float4 (every
+// pointer 16-byte aligned, checked on the host), the tail [4 n4, n) one float at a time.
+struct DpmScalars {
+  float g, alpha, sigma, cx, k0, k1, k2;
+};
+
+__device__ __forceinline__ void dpm_element(float x, float ec, float eu, float m1, float m2, bool cfg, const DpmScalars& s,
+                                            float& m0, float& xp) {
+  float e = ec;
+  if (cfg) e = eu + s.g * (ec - eu);
+  m0 = (x - s.sigma * e) / s.alpha;
+  xp = s.cx * x + s.k0 * m0 + s.k1 * m1 + s.k2 * m2;
+}
+
+__global__ void __launch_bounds__(256) dpm_update_kernel(const float* __restrict__ x, const float* __restrict__ ec, const float* __restrict__ eu,
+                                                         const float* __restrict__ m1, const float* __restrict__ m2, DpmScalars s,
+                                                         float* __restrict__ x0_out, float* __restrict__ x_prev, long long n4, long long n) {
+  pdl_trigger();
+  pdl_wait();
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool cfg = eu != nullptr;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (long long i = tid; i < n4; i += stride) {
+    const float4 xv = __ldg(reinterpret_cast<const float4*>(x) + i);
+    const float4 cv = __ldg(reinterpret_cast<const float4*>(ec) + i);
+    const float4 uv = cfg ? __ldg(reinterpret_cast<const float4*>(eu) + i) : zero;
+    const float4 p1 = m1 ? __ldg(reinterpret_cast<const float4*>(m1) + i) : zero;
+    const float4 p2 = m2 ? __ldg(reinterpret_cast<const float4*>(m2) + i) : zero;
+    float4 m0, xp;
+    dpm_element(xv.x, cv.x, uv.x, p1.x, p2.x, cfg, s, m0.x, xp.x);
+    dpm_element(xv.y, cv.y, uv.y, p1.y, p2.y, cfg, s, m0.y, xp.y);
+    dpm_element(xv.z, cv.z, uv.z, p1.z, p2.z, cfg, s, m0.z, xp.z);
+    dpm_element(xv.w, cv.w, uv.w, p1.w, p2.w, cfg, s, m0.w, xp.w);
+    reinterpret_cast<float4*>(x0_out)[i] = m0;
+    reinterpret_cast<float4*>(x_prev)[i] = xp;
+  }
+  for (long long i = 4 * n4 + tid; i < n; i += stride) {
+    float m0, xp;
+    dpm_element(x[i], ec[i], cfg ? eu[i] : 0.f, m1 ? m1[i] : 0.f, m2 ? m2[i] : 0.f, cfg, s, m0, xp);
+    x0_out[i] = m0;
+    x_prev[i] = xp;
+  }
+}
+
 }  // namespace glg
 
 namespace glg {
@@ -509,4 +554,20 @@ extern "C" int glg_sampler_update(const float* x, const float* e_cond, const flo
                                                             sqrtf(a_t), sqrtf(1.f - a_t), sqrtf(a_prev), sqrtf(1.f - a_prev), e_out, x_prev, n);
   count_launch();
   return check_launch("sampler_update launch");
+}
+
+extern "C" int glg_dpm_update(const float* x, const float* e_cond, const float* e_uncond, float guidance, const float* m1, const float* m2,
+                              float alpha, float sigma, float cx, float k0, float k1, float k2, float* x0_out, float* x_prev, int64_t n,
+                              void* stream) {
+  if (!x || !e_cond || !x0_out || !x_prev) return set_error("glg_dpm_update: x, e_cond, x0_out and x_prev are required");
+  if (n < 0) return set_error("glg_dpm_update: n must be >= 0");
+  if (n == 0) return 0;
+  const uintptr_t bits = (uintptr_t)x | (uintptr_t)e_cond | (uintptr_t)e_uncond | (uintptr_t)m1 | (uintptr_t)m2 | (uintptr_t)x0_out |
+                         (uintptr_t)x_prev;
+  const long long n4 = (bits & 15) ? 0 : n / 4;          // a misaligned view takes the scalar path for all of n
+  const DpmScalars s{guidance, alpha, sigma, cx, k0, k1, k2};
+  const unsigned grid = blocks_for(n4 > 0 ? n4 : n, 256);
+  launch_k(dpm_update_kernel, dim3(grid > 4096 ? 4096 : grid), dim3(256), 0, ST, 1, x, e_cond, e_uncond, m1, m2, s, x0_out, x_prev, n4, (long long)n);
+  count_launch();
+  return check_launch("dpm_update launch");
 }

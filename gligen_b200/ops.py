@@ -388,3 +388,14 @@ class CudaOps:
                                             float(a_t), float(a_prev), _ptr(e_out), x_prev.data_ptr(), x.numel(), self._stream()),
                 "glg_sampler_update")
         self._note("sampler_update")
+
+    def dpm_update(self, x, e_cond, e_uncond, guidance, m1, m2, alpha, sigma, coefs, x0_out, x_prev):
+        """One DPM-Solver++ step (glg_dpm_update): x0_out = (x - sigma e) / alpha, x_prev = cx x + k0 x0_out + k1 m1 + k2 m2 with
+        coefs = (cx, k0, k1, k2); e the CFG mix of e_cond / e_uncond; m1, m2 may be None.  Outputs alias no input."""
+        for t in (x, e_cond, e_uncond, m1, m2, x0_out, x_prev):
+            assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == x.numel())
+        L.check(self._c.glg_dpm_update(x.data_ptr(), e_cond.data_ptr(), _ptr(e_uncond), float(guidance), _ptr(m1), _ptr(m2),
+                                        float(alpha), float(sigma), float(coefs[0]), float(coefs[1]), float(coefs[2]), float(coefs[3]),
+                                        x0_out.data_ptr(), x_prev.data_ptr(), x.numel(), self._stream()),
+                "glg_dpm_update")
+        self._note("dpm_update")

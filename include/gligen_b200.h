@@ -249,6 +249,22 @@ int glg_sampler_update(const float* x, const float* e_cond, const float* e_uncon
                        float c0, float c1, float c2, float c3,
                        float a_t, float a_prev, float* e_out, float* x_prev, int64_t n, void* stream);
 
+/* ---- DPM-Solver++ multistep update (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion
+ * Probabilistic Models", Algorithm 2), one fused fp32 kernel --------------------------------------------------------------
+ * e      = e_u + g*(e_c - e_u)                       (if e_uncond != NULL, else e = e_cond)
+ * x0_out = m0 = (x - sigma*e) / alpha                 data prediction at the evaluated timestep s0
+ * x_prev = cx*x + k0*m0 + k1*m1 + k2*m2               (m1, m2 nullable: the two previous data predictions, read as 0)
+ * alpha = sqrt(ac_s0), sigma = sqrt(1 - ac_s0).  With lambda = log(alpha/sigma), h = lambda_t - lambda_s0,
+ * r0 = (lambda_s0 - lambda_s1)/h, r1 = (lambda_s1 - lambda_s2)/h, phi = -alpha_t expm1(-h), D1_0 = (m0 - m1)/r0,
+ * D1_1 = (m1 - m2)/r1, the host expands into (cx, k0, k1, k2) (in float64, passed as fp32):
+ *   order 1:  x_t = (sigma_t/sigma_s0) x + phi m0                                        (DDIM, eta = 0)
+ *   order 2:  x_t = (sigma_t/sigma_s0) x + phi (m0 + D1_0/2)
+ *   order 3:  x_t = (sigma_t/sigma_s0) x + phi m0 + alpha_t (expm1(-h)/h + 1) D1 - alpha_t ((expm1(-h) + h)/h^2 - 1/2) D2,
+ *             D1 = D1_0 + r0/(r0 + r1) (D1_0 - D1_1), D2 = (D1_0 - D1_1)/(r0 + r1).
+ * x0_out and x_prev must not alias any input or each other.  Any n >= 0; 16-byte-aligned pointers take 16-byte accesses. */
+int glg_dpm_update(const float* x, const float* e_cond, const float* e_uncond, float guidance, const float* m1, const float* m2,
+                   float alpha, float sigma, float cx, float k0, float k1, float k2, float* x0_out, float* x_prev, int64_t n, void* stream);
+
 /* ---- engine level: a whole UNet forward from an exported plan ----------------------------------
  * Replaces UNetModel.forward (openaimodel.py:420-464) for hosts that cannot embed Python.  gligen_b200/export.py writes one
  * (batch rows, grounding slots, context length) plan of the engine to a file: packed weights, workspace sizes and the ordered
