@@ -108,7 +108,9 @@ __device__ __forceinline__ float act_f(int act, float v) {
 // The epilogue walks 32-column chunks and issues every global load of a chunk (bias, LayerNorm column sums, row bias,
 // residual; both rows of the thread) before the chunk's first store: the compiler cannot move a load across a store that
 // may alias it, so loads interleaved with stores would cost one L2 round trip per 8 columns.
-template <int BN, bool GEGLU>
+// ACT = false compiles the activation out: the fully unrolled epilogue is instruction-fetch bound, and the inlined
+// SiLU / GELU / quick-GELU branches of every element (which no UNet projection takes) cost the GEMMs 14 % of their time.
+template <int BN, bool GEGLU, bool ACT>
 __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float (&d)[BN / 2], int row_base, int n_blk, float gate, int lane) {
   const int cq = 2 * (lane & 3);
   int row[2]; bool row_ok[2]; size_t out_off[2];
@@ -199,7 +201,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float (&d)[B
             v1 = fmaf(v1, ln_rstd[hr], fmaf(cs[jj].y, c1[hr], bias[jj].y));
           } else if (p.bias) { v0 += bias[jj].x; v1 += bias[jj].y; }
           if (rb[hr]) { v0 += rbv[hr][jj].x; v1 += rbv[hr][jj].y; }
-          v0 = act_f(p.act, v0); v1 = act_f(p.act, v1);
+          if constexpr (ACT) { v0 = act_f(p.act, v0); v1 = act_f(p.act, v1); }
           if (p.gate) { v0 *= gate; v1 *= gate; }
           if (p.residual && row_ok[hr]) {
             const float2 r = unpack_bf16x2(res[hr][jj]);
@@ -472,7 +474,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int mh = 0; mh < MH; ++mh) {
         const int row_base = m_blk * ROWS_PER_TILE + (int)rank * 128 + (PP ? mh : cw) * 64 + (warp & 3) * 16 + (lane >> 2);
         if (p.splits > 1) epilogue_partial<BN>(p, d[mh], row_base, n_blk, split, lane);
-        else epilogue_tile<BN, GEGLU>(p, d[mh], row_base, n_blk, gate, lane);
+        else if (!GEGLU && p.act) epilogue_tile<BN, GEGLU, true>(p, d[mh], row_base, n_blk, gate, lane);
+        else epilogue_tile<BN, GEGLU, false>(p, d[mh], row_base, n_blk, gate, lane);
       }
     }
   }
