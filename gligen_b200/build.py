@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libgligen_b200.so")
-SOURCES = ["capi.cu", "engine_capi.cu", "tma_host.cu", "gemm_tc.cu", "attention.cu", "norm.cu", "elementwise.cu", "frontend.cu", "fuser.cu"]
+SOURCES = ["capi.cu", "engine_capi.cu", "tma_host.cu", "gemm_tc.cu", "gemm_tc_bn64.cu", "gemm_tc_bn128.cu", "gemm_tc_bn160.cu", "gemm_tc_bn256.cu", "attention.cu", "norm.cu", "elementwise.cu", "frontend.cu", "fuser.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",

@@ -1,0 +1,8 @@
+// The gemm_tc_kernel instantiations of 256-wide tiles (gemm_tc.cuh: GLG_GEMM_INSTANCES_BN256); one unit per tile width
+// keeps each compile short and lets them build in parallel.
+#define GLG_GEMM_KERNEL_UNIT
+#include "gemm_tc.cuh"
+
+namespace glg {
+GLG_GEMM_INSTANCES_BN256(GLG_GEMM_INSTANTIATE)
+}  // namespace glg

@@ -87,7 +87,7 @@ SIGNATURES = {
                                c_float, c_float, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_int64, c_void_p]),
 }
 # not part of the public header: test hook
-_DEBUG_SIGNATURES = {"glg_debug_force_bn": (None, [c_int]), "glg_debug_pick_tile": (None, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64, C.POINTER(c_int)]), "glg_debug_attn_mode": (None, [c_int]), "glg_debug_attn_poly_share": (None, [c_int]), "glg_debug_gemm_cta2": (None, [c_int]), "glg_debug_splitk": (None, [c_int]), "glg_debug_gemm_bres": (None, [c_int]), "glg_debug_gemm_pp": (None, [c_int]), "glg_debug_pick_pingpong": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64])}
+_DEBUG_SIGNATURES = {"glg_debug_force_bn": (None, [c_int]), "glg_debug_pick_tile": (None, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64, C.POINTER(c_int)]), "glg_debug_attn_mode": (None, [c_int]), "glg_debug_attn_poly_share": (None, [c_int]), "glg_debug_gemm_cta2": (None, [c_int]), "glg_debug_splitk": (None, [c_int]), "glg_debug_gemm_bres": (None, [c_int]), "glg_debug_gemm_pp": (None, [c_int]), "glg_debug_pick_pingpong": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64]), "glg_debug_epilogue_kind": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_int])}
 
 _lib: Optional[C.CDLL] = None
 
