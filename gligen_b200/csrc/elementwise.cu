@@ -390,6 +390,60 @@ __global__ void __launch_bounds__(256) dpm_update_kernel(const float* __restrict
   }
 }
 
+// One UniPC step (include/gligen_b200.h, glg_unipc_update): the corrector for the point just evaluated, then the predictor
+// from the corrected state.  Elements [0, 4 n4) move as float4 (every pointer 16-byte aligned, checked on the host), the tail
+// [4 n4, n) one float at a time.
+struct UniPCScalars {
+  float g, alpha, sigma, cc, c0, c1, c2, c3, pc, p0, p1, p2;
+};
+
+__device__ __forceinline__ void unipc_element(float x, float xcp, float ec, float eu, float m1, float m2, float m3, bool cfg, bool corr,
+                                              const UniPCScalars& s, float& m0, float& xc, float& xn) {
+  float e = ec;
+  if (cfg) e = eu + s.g * (ec - eu);
+  m0 = (x - s.sigma * e) / s.alpha;
+  xc = corr ? s.cc * xcp + s.c0 * m0 + s.c1 * m1 + s.c2 * m2 + s.c3 * m3 : x;
+  xn = s.pc * xc + s.p0 * m0 + s.p1 * m1 + s.p2 * m2;
+}
+
+__global__ void __launch_bounds__(256) unipc_update_kernel(const float* __restrict__ x, const float* __restrict__ xcp,
+                                                           const float* __restrict__ ec, const float* __restrict__ eu,
+                                                           const float* __restrict__ m1, const float* __restrict__ m2,
+                                                           const float* __restrict__ m3, UniPCScalars s, float* __restrict__ m_out,
+                                                           float* __restrict__ xc_out, float* __restrict__ x_next, long long n4, long long n) {
+  pdl_trigger();
+  pdl_wait();
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool cfg = eu != nullptr, corr = xcp != nullptr;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (long long i = tid; i < n4; i += stride) {
+    const float4 xv = __ldg(reinterpret_cast<const float4*>(x) + i);
+    const float4 cp = corr ? __ldg(reinterpret_cast<const float4*>(xcp) + i) : zero;
+    const float4 cv = __ldg(reinterpret_cast<const float4*>(ec) + i);
+    const float4 uv = cfg ? __ldg(reinterpret_cast<const float4*>(eu) + i) : zero;
+    const float4 h1 = m1 ? __ldg(reinterpret_cast<const float4*>(m1) + i) : zero;
+    const float4 h2 = m2 ? __ldg(reinterpret_cast<const float4*>(m2) + i) : zero;
+    const float4 h3 = m3 ? __ldg(reinterpret_cast<const float4*>(m3) + i) : zero;
+    float4 m0, xc, xn;
+    unipc_element(xv.x, cp.x, cv.x, uv.x, h1.x, h2.x, h3.x, cfg, corr, s, m0.x, xc.x, xn.x);
+    unipc_element(xv.y, cp.y, cv.y, uv.y, h1.y, h2.y, h3.y, cfg, corr, s, m0.y, xc.y, xn.y);
+    unipc_element(xv.z, cp.z, cv.z, uv.z, h1.z, h2.z, h3.z, cfg, corr, s, m0.z, xc.z, xn.z);
+    unipc_element(xv.w, cp.w, cv.w, uv.w, h1.w, h2.w, h3.w, cfg, corr, s, m0.w, xc.w, xn.w);
+    reinterpret_cast<float4*>(m_out)[i] = m0;
+    reinterpret_cast<float4*>(xc_out)[i] = xc;
+    reinterpret_cast<float4*>(x_next)[i] = xn;
+  }
+  for (long long i = 4 * n4 + tid; i < n; i += stride) {
+    float m0, xc, xn;
+    unipc_element(x[i], corr ? xcp[i] : 0.f, ec[i], cfg ? eu[i] : 0.f, m1 ? m1[i] : 0.f, m2 ? m2[i] : 0.f, m3 ? m3[i] : 0.f, cfg, corr, s,
+                  m0, xc, xn);
+    m_out[i] = m0;
+    xc_out[i] = xc;
+    x_next[i] = xn;
+  }
+}
+
 }  // namespace glg
 
 namespace glg {
@@ -570,4 +624,22 @@ extern "C" int glg_dpm_update(const float* x, const float* e_cond, const float* 
   launch_k(dpm_update_kernel, dim3(grid > 4096 ? 4096 : grid), dim3(256), 0, ST, 1, x, e_cond, e_uncond, m1, m2, s, x0_out, x_prev, n4, (long long)n);
   count_launch();
   return check_launch("dpm_update launch");
+}
+
+extern "C" int glg_unipc_update(const float* x, const float* xc_prev, const float* e_cond, const float* e_uncond, float guidance,
+                                const float* m1, const float* m2, const float* m3, float alpha, float sigma, float cc, float c0, float c1,
+                                float c2, float c3, float pc, float p0, float p1, float p2, float* m_out, float* xc_out, float* x_next,
+                                int64_t n, void* stream) {
+  if (!x || !e_cond || !m_out || !xc_out || !x_next) return set_error("glg_unipc_update: x, e_cond, m_out, xc_out and x_next are required");
+  if (n < 0) return set_error("glg_unipc_update: n must be >= 0");
+  if (n == 0) return 0;
+  const uintptr_t bits = (uintptr_t)x | (uintptr_t)xc_prev | (uintptr_t)e_cond | (uintptr_t)e_uncond | (uintptr_t)m1 | (uintptr_t)m2 |
+                         (uintptr_t)m3 | (uintptr_t)m_out | (uintptr_t)xc_out | (uintptr_t)x_next;
+  const long long n4 = (bits & 15) ? 0 : n / 4;          // a misaligned view takes the scalar path for all of n
+  const UniPCScalars s{guidance, alpha, sigma, cc, c0, c1, c2, c3, pc, p0, p1, p2};
+  const unsigned grid = blocks_for(n4 > 0 ? n4 : n, 256);
+  launch_k(unipc_update_kernel, dim3(grid > 4096 ? 4096 : grid), dim3(256), 0, ST, 1, x, xc_prev, e_cond, e_uncond, m1, m2, m3, s, m_out,
+           xc_out, x_next, n4, (long long)n);
+  count_launch();
+  return check_launch("unipc_update launch");
 }

@@ -399,3 +399,16 @@ class CudaOps:
                                         x0_out.data_ptr(), x_prev.data_ptr(), x.numel(), self._stream()),
                 "glg_dpm_update")
         self._note("dpm_update")
+
+    def unipc_update(self, x, xc_prev, e_cond, e_uncond, guidance, m1, m2, m3, alpha, sigma, coefs, m_out, xc_out, x_next):
+        """One UniPC step (glg_unipc_update): m_out = (x - sigma e) / alpha, xc_out = cc xc_prev + c0 m_out + c1 m1 + c2 m2 + c3 m3
+        (xc_out = x when xc_prev is None), x_next = pc xc_out + p0 m_out + p1 m1 + p2 m2 with coefs = (cc, c0, c1, c2, c3, pc, p0,
+        p1, p2); e the CFG mix of e_cond / e_uncond; m1, m2, m3 may be None.  Outputs alias no input."""
+        assert len(coefs) == 9
+        for t in (x, xc_prev, e_cond, e_uncond, m1, m2, m3, m_out, xc_out, x_next):
+            assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == x.numel())
+        L.check(self._c.glg_unipc_update(x.data_ptr(), _ptr(xc_prev), e_cond.data_ptr(), _ptr(e_uncond), float(guidance), _ptr(m1),
+                                          _ptr(m2), _ptr(m3), float(alpha), float(sigma), *(float(c) for c in coefs),
+                                          m_out.data_ptr(), xc_out.data_ptr(), x_next.data_ptr(), x.numel(), self._stream()),
+                "glg_unipc_update")
+        self._note("unipc_update")

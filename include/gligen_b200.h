@@ -265,6 +265,26 @@ int glg_sampler_update(const float* x, const float* e_cond, const float* e_uncon
 int glg_dpm_update(const float* x, const float* e_cond, const float* e_uncond, float guidance, const float* m1, const float* m2,
                    float alpha, float sigma, float cx, float k0, float k1, float k2, float* x0_out, float* x_prev, int64_t n, void* stream);
 
+/* ---- UniPC predictor-corrector update (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework for Fast Sampling
+ * of Diffusion Models"; data prediction, B(h) = expm1(-h)), one fused fp32 kernel per step i ------------------------------
+ * e      = e_u + g*(e_c - e_u)                                      (if e_uncond != NULL, else e = e_cond)
+ * m_out  = m0 = (x - sigma*e) / alpha                                data prediction at point i (x = x_i)
+ * xc_out = xc = cc*xc_prev + c0*m0 + c1*m1 + c2*m2 + c3*m3           UniC from point i-1 (xc_prev NULL: xc = x, the first step)
+ * x_next = pc*xc + p0*m0 + p1*m1 + p2*m2                             UniP to point i+1, from the fp32 xc stored in xc_out
+ * m1, m2, m3 (nullable, read as 0): the data predictions at points i-1, i-2, i-3.  alpha = sqrt(ac_i), sigma = sqrt(1 - ac_i).
+ * With lambda = log(alpha/sigma), a step from s to t of order p has h = lambda_t - lambda_s, B = expm1(-h),
+ * r_k = (lambda_{s-k} - lambda_s)/h, D_k = (m_{s-k} - m_s)/r_k (k < p), r_p = 1, R[a] = (r_1 .. r_p)^a and
+ * b[a] = g_{a+1} (a+1)!/B with g_1 = B/(-h) - 1, g_{a+1} = g_a/(-h) - 1/(a+1)!; the host expands in float64 (passed as fp32)
+ *   UniP:  x_t = (sigma_t/sigma_s) x_s - alpha_t B m_s - alpha_t B sum_k rhoP_k D_k
+ *          rhoP = [] (p = 1), [1/2] (p = 2: DPM-Solver++ 2M), solve(R[:2,:2], b[:2]) (p = 3)
+ *   UniC:  x_t = (sigma_t/sigma_s) x_s - alpha_t B m_s - alpha_t B (sum_{k<p} rhoC_k D_k + rhoC_p (m_t - m_s))
+ *          rhoC = [1/2] (p = 1), solve(R, b) (p >= 2).
+ * The outputs must not alias any input or each other.  Any n >= 0; 16-byte-aligned pointers take 16-byte accesses. */
+int glg_unipc_update(const float* x, const float* xc_prev, const float* e_cond, const float* e_uncond, float guidance,
+                     const float* m1, const float* m2, const float* m3, float alpha, float sigma,
+                     float cc, float c0, float c1, float c2, float c3, float pc, float p0, float p1, float p2,
+                     float* m_out, float* xc_out, float* x_next, int64_t n, void* stream);
+
 /* ---- engine level: a whole UNet forward from an exported plan ----------------------------------
  * Replaces UNetModel.forward (openaimodel.py:420-464) for hosts that cannot embed Python.  gligen_b200/export.py writes one
  * (batch rows, grounding slots, context length) plan of the engine to a file: packed weights, workspace sizes and the ordered

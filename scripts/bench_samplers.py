@@ -1,4 +1,5 @@
-"""Images/s of the samplers on one GPU: PLMS-50 against DPM-Solver++ 2M at 20 and 25 steps.
+"""Images/s of the samplers on one GPU: PLMS-50 against DPM-Solver++ 2M at 20 and 25 steps, and UniPC-2 at 10 and 15 steps
+against DPM-Solver++ 2M at 10 (the same number of passes).
 
     python scripts/bench_samplers.py [--repeats 2] [--batch 4]
 
@@ -7,7 +8,10 @@ alpha_type [0.3, 0, 0.7] (gligen_inference's default: the fusers are on for the 
 1. Every sampler once untimed, then the samplers alternately, `--repeats` times each: wall time of sample() between device
    synchronisations -> images/s, and the UNet passes per image (one CFG-batched pass evaluates cond and uncond).
 2. glg_dpm_update alone, CUDA events around a CUDA graph of 200 launches at the batch's latent (4 x 4 x 64 x 64, CFG, order 2), against its HBM
-   bound: x, e_c, e_u, m1 read and x0_out, x_prev written, over 3.35 TB/s (H100 SXM data sheet).
+   bound: x, e_c, e_u, m1 read and x0_out, x_prev written, over 3.35 TB/s (H100 SXM data sheet).  Likewise glg_unipc_update
+   (order 3, a step that reads all three earlier data predictions): x, xc_prev, e_c, e_u, m1, m2, m3 read and m_out, xc_out,
+   x_next written.  The UniPC rows must take exactly one UNet pass per image and step of the DDIM uniform grid (S of them, but
+   16 at S = 15: the grid's spacing is 1000 // S); the script stops if one does not.
 3. A diagnostic, not a quality measure: the rel-L2 distance of each sampler's final latent from a DPM-Solver++ 3M run at 250
    steps on the same seeded inputs.  That run is not a converged solution (the DDIM grid's last step, t = 1 -> alphas_cumprod[0],
    has the same size at every S), and with synthetic weights the distance says how the solvers differ, not how the images look.
@@ -32,30 +36,23 @@ from bench_fusers import HBM_BYTES_PER_S, card  # noqa: E402
 
 DEV = "cuda:0"
 ALPHA_TYPE = [0.3, 0.0, 0.7]
-RUNS = [("PLMS-50", "plms", 50, None), ("DPM-Solver++ 2M-20", "dpm", 20, 2), ("DPM-Solver++ 2M-25", "dpm", 25, 2)]
+RUNS = [("PLMS-50", "plms", 50, None), ("DPM-Solver++ 2M-20", "dpm", 20, 2), ("DPM-Solver++ 2M-25", "dpm", 25, 2),
+        ("UniPC-2 10", "unipc", 10, 2), ("UniPC-2 15", "unipc", 15, 2), ("DPM-Solver++ 2M-10", "dpm", 10, 2)]
 REFERENCE_RUN = ("DPM-Solver++ 3M-250", "dpm", 250, 3)
 
 
-def update_kernel_time(batch, reps=200):
-    from gligen_b200.ops import CudaOps
-    from ldm.models.diffusion import dpm_solver as DS
-    import numpy as np
-    from oracle import sampler_oracle as SO
-    ops = CudaOps(DEV)
-    x, ec, eu, m1 = (torch.randn(batch, 4, 64, 64, device=DEV) for _ in range(4))
-    m0, xp = torch.empty_like(x), torch.empty_like(x)
-    alpha, sigma = DS.grid_alpha_sigma(SO.make_schedule()["alphas_cumprod"], np.flip(SO.ddim_timesteps(20)))
-    coefs = DS.step_coefficients(alpha, sigma, DS.step_orders(len(alpha) - 1, 2))[5]
+def _graph_time(name, batch, launch, nbytes, reps=200):
+    """CUDA events around a CUDA graph of `reps` launch() calls -> us per launch, against the HBM bound of nbytes."""
     # the launches are captured in a CUDA graph: issued one by one from Python, the ctypes call takes longer than the kernel and
     # the events would time the host
     stream = torch.cuda.Stream()
     with torch.cuda.stream(stream):
         for _ in range(20):
-            ops.dpm_update(x, ec, eu, 7.5, m1, None, alpha[5], sigma[5], coefs, m0, xp)
+            launch()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph, stream=stream):
             for _ in range(reps):
-                ops.dpm_update(x, ec, eu, 7.5, m1, None, alpha[5], sigma[5], coefs, m0, xp)
+                launch()
     graph.replay()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -64,11 +61,43 @@ def update_kernel_time(batch, reps=200):
     e1.record()
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / reps
-    nbytes = 6 * x.numel() * 4
     bound_us = nbytes / HBM_BYTES_PER_S * 1e6
-    print(f"glg_dpm_update {batch} x 4 x 64 x 64: {us:.2f} us, {nbytes / 1e6:.2f} MB -> {nbytes / us / 1e3:.0f} GB/s; "
+    print(f"{name} {batch} x 4 x 64 x 64: {us:.2f} us, {nbytes / 1e6:.2f} MB -> {nbytes / us / 1e3:.0f} GB/s; "
           f"HBM bound {bound_us:.2f} us, {us / bound_us:.2f}x the bound", flush=True)
     return dict(us=us, bound_us=bound_us, mb=nbytes / 1e6)
+
+
+def _step20_grid():
+    from ldm.models.diffusion import dpm_solver as DS
+    import numpy as np
+    from oracle import sampler_oracle as SO
+    return DS.grid_alpha_sigma(SO.make_schedule()["alphas_cumprod"], np.flip(SO.ddim_timesteps(20)))
+
+
+def update_kernel_time(batch):
+    from gligen_b200.ops import CudaOps
+    from ldm.models.diffusion import dpm_solver as DS
+    ops = CudaOps(DEV)
+    x, ec, eu, m1 = (torch.randn(batch, 4, 64, 64, device=DEV) for _ in range(4))
+    m0, xp = torch.empty_like(x), torch.empty_like(x)
+    alpha, sigma = _step20_grid()
+    coefs = DS.step_coefficients(alpha, sigma, DS.step_orders(len(alpha) - 1, 2))[5]
+    return _graph_time("glg_dpm_update", batch, lambda: ops.dpm_update(x, ec, eu, 7.5, m1, None, alpha[5], sigma[5], coefs, m0, xp),
+                       6 * x.numel() * 4)
+
+
+def unipc_update_kernel_time(batch):
+    from gligen_b200.ops import CudaOps
+    from ldm.models.diffusion import dpm_solver as DS
+    from ldm.models.diffusion import unipc as UP
+    ops = CudaOps(DEV)
+    x, xcp, ec, eu, m1, m2, m3 = (torch.randn(batch, 4, 64, 64, device=DEV) for _ in range(7))
+    m0, xc, xn = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
+    alpha, sigma = _step20_grid()
+    coefs = UP.step_coefficients(alpha, sigma, DS.step_orders(len(alpha) - 1, 3))[5]
+    return _graph_time("glg_unipc_update", batch,
+                       lambda: ops.unipc_update(x, xcp, ec, eu, 7.5, m1, m2, m3, alpha[5], sigma[5], coefs, m0, xc, xn),
+                       10 * x.numel() * 4)
 
 
 def main():
@@ -84,6 +113,8 @@ def main():
     from ldm.models.diffusion.dpm_solver import DPMSolverSampler
     from ldm.models.diffusion.ldm import LatentDiffusion
     from ldm.models.diffusion.plms import PLMSSampler
+    from ldm.models.diffusion.unipc import UniPCSampler
+    from ldm.modules.diffusionmodules.util import make_ddim_timesteps
 
     print(card(), flush=True)
     cfg, model = build_model("sd14_box_text", DEV)
@@ -105,7 +136,12 @@ def main():
     def run(kind, S, order):
         model.load_state_dict(weights)
         model.engine()                                  # re-pack the weights outside the timed window
-        sampler = PLMSSampler(diffusion, model, **kw) if kind == "plms" else DPMSolverSampler(diffusion, model, order=order, **kw)
+        if kind == "plms":
+            sampler = PLMSSampler(diffusion, model, **kw)
+        elif kind == "dpm":
+            sampler = DPMSolverSampler(diffusion, model, order=order, **kw)
+        else:
+            sampler = UniPCSampler(diffusion, model, order=order, **kw)
         input, _, _ = sampler_inputs(cfg, model, dinp, dbatch)
         passes["n"] = 0
         torch.manual_seed(1234)
@@ -121,6 +157,9 @@ def main():
         latents, times, npass = {}, {name: [] for name, *_ in RUNS}, {}
         for name, kind, S, order in RUNS:               # warm-up: every shape and schedule once
             _, npass[name], latents[name] = run(kind, S, order)
+            steps = len(make_ddim_timesteps("uniform", S, 1000, verbose=False))
+            if kind == "unipc" and npass[name] != steps:
+                raise SystemExit(f"{name}: {npass[name]} UNet passes per image, expected one per step of the grid ({steps})")
         for _ in range(a.repeats):
             for name, kind, S, order in RUNS:
                 secs, n, lat = run(kind, S, order)
@@ -146,7 +185,9 @@ def main():
     finally:
         os.chdir(cwd)
     kern = update_kernel_time(a.batch)
-    print(json.dumps(dict(card=card(), batch=a.batch, alpha_type=ALPHA_TYPE, guidance=7.5, samplers=results, dpm_update=kern)))
+    ukern = unipc_update_kernel_time(a.batch)
+    print(json.dumps(dict(card=card(), batch=a.batch, alpha_type=ALPHA_TYPE, guidance=7.5, samplers=results, dpm_update=kern,
+                          unipc_update=ukern)))
 
 
 if __name__ == "__main__":
