@@ -36,7 +36,7 @@ int main(int argc, char** argv) {
   if (argc < 3) { fprintf(stderr, "usage: %s plan.glgplan out.bin [name=file.bin ...] [fuser=0|1]\n", argv[0]); return 2; }
   if (glg_abi_version() != GLG_ABI_VERSION) { fprintf(stderr, "unet_host: header / library ABI mismatch\n"); return 1; }
   GlgEngine* e = NULL;
-  if (glg_engine_load(argv[1], &e)) die("glg_engine_load");
+  if (glg_engine_load(argv[1], &e)) die(argv[1]);          /* a refused plan: the message names the op and what is wrong */
   int fuser_on = 1;
   for (int i = 3; i < argc; ++i) {
     char* eq = strchr(argv[i], '=');

@@ -292,6 +292,9 @@ int glg_unipc_update(const float* x, const float* xc_prev, const float* e_cond, 
  * [rows], "in:context" fp32 [rows,77,768], "in:coords" / "in:masks" / "in:feat0" / "in:fmask0" (/ "in:feat1" / "in:fmask1",
  * "in:extra") as GroundingNetInput.prepare lays them out, "out" fp32 [rows,C,H,W]; weights "W:<name>" ("W:gates" holds
  * scale * tanh(alpha) per fuser, "W:conv_in.w" / "W:conv_in.b" the first conv that restore_first_conv_from_SD swaps).
+ * glg_engine_load checks every op of the file against the calls above (name, argument count and kinds, struct sizes, every pointer
+ * inside its buffer) before it allocates anything; a plan that fails a check is refused (< 0, glg_last_error names the op index and
+ * the problem) and glg_engine_run only ever replays checked ops.
  * Not thread-safe per handle; all work is enqueued on `stream`; CUDA-graph capturable (no allocation inside run). */
 typedef struct GlgEngine GlgEngine;
 int glg_engine_load(const char* path, GlgEngine** out);

@@ -26,6 +26,31 @@ def test_library_exports_every_declared_symbol():
     assert L.glg_launch_count() == 0
 
 
+def test_engine_loader_op_table_matches_header():
+    """glg_engine_load checks every op of a plan file against the table in csrc/engine_capi.cu.  Each entry's argument tags must
+    be the ones gligen_b200/export.py writes for that function's declaration (lib.SIGNATURES), or plans using it are refused."""
+    import ctypes as C
+    from gligen_b200 import lib
+    src = open(os.path.join(ROOT, "gligen_b200", "csrc", "engine_capi.cu")).read()
+    table = re.findall(r'\{"(glg_\w+)", "([A-Z]+)", (0|sizeof\(\w+\)),', src)
+    names = [n for n, _, _ in table]
+    assert len(names) == len(set(names)) and {"glg_gemm", "glg_attention", "glg_groupnorm", "glg_grid_resample_gate"} <= set(names)
+    for name, tags, sbytes in table:
+        argtypes = lib.SIGNATURES[name][1]
+        want = ""
+        for i, ty in enumerate(argtypes):
+            target = getattr(ty, "_type_", None)
+            if isinstance(target, type) and issubclass(target, C.Structure):
+                want += "S"
+                assert sbytes == f"sizeof({target.__name__})", (name, sbytes)
+            elif ty is C.c_void_p:
+                want += "T" if i == len(argtypes) - 1 else "P"
+            else:
+                want += "F" if ty is C.c_float else "I"
+        assert tags == want, (name, tags, want)
+        assert ("S" in tags) == (sbytes != "0"), (name, sbytes)
+
+
 def test_kernels_are_hopper_native():
     """SASS evidence: wgmma -> HGMMA, TMA loads -> UTMALDG (incl. the multicast of the paired GEMM), mma.sync -> HMMA."""
     import shutil

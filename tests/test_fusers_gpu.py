@@ -160,9 +160,9 @@ def test_scale_zero_equals_gated_sa(name):
 
 @pytest.mark.parametrize("name,max_objs,scales", [("tiny_gated_ca", 6, (1.0, 0.0)), ("tiny_hed_gated_sa2", 0, (1.0,))])
 def test_exported_plan_matches_python_engine(name, max_objs, scales, tmp_path):
-    """gatedCA and gatedSA2 plans replayed by the library alone (glg_engine_*), bit for bit.  The replay helper drives the scale
-    through set_alpha_scale, which leaves gatedSA2 fusers at 1 (as in the reference), so that model is replayed at scale 1 only."""
-    from test_native_engine_gpu import _case
+    """gatedCA and gatedSA2 plans replayed by the library alone (glg_engine_*), bit for bit (every fuser variant, its other scales
+    and SD-sized models: tests/test_native_engine_variants_gpu.py)."""
+    from native_plan import _case
     info = _case(name, 2, max_objs, tmp_path, scales=scales)
     assert info["ops"] > 300
 

@@ -7,70 +7,12 @@ import pytest
 import torch
 
 from gligen_b200 import synth
-from gligen_b200.export import NativePlan, export_plan
-from gligen_b200.pipeline import build_model, set_alpha_scale, to_device
+from gligen_b200.export import export_plan
+from gligen_b200.pipeline import build_model, to_device
+from native_plan import _case
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _case(name, B, max_objs, tmp_path, scales=(1.0, 0.0), map_size=None):
-    cfg, model = build_model(name, DEV)
-    inp = synth.make_inputs(cfg, B, max_objs, seed=4, map_size=map_size)
-    ts = torch.tensor([981, 401, 21, 1][:B], dtype=torch.long, device=DEV)
-    x, ctx, uc = inp["x"].to(DEV), inp["context"].to(DEV), inp["uc"].to(DEV)
-    batch = to_device(inp["batch"], DEV)
-    grounding = model.grounding_tokenizer_input.prepare(batch)
-    extra = None
-    if cfg.inpaint_mode:
-        from inpaint_mask_func import draw_masks_from_boxes
-        mask = draw_masks_from_boxes(batch["boxes"], cfg.image_size).to(DEV)
-        extra = torch.cat([inp["z0"].to(DEV) * mask, mask], dim=1)
-    eng = model.engine()
-    gextra = None
-    if cfg.spatial:
-        from gligen_b200.spec import SPATIAL_MAP_KEY
-        gmap = batch[SPATIAL_MAP_KEY[cfg.tokenizer]]
-        gextra = gmap
-        eng._n_objs(grounding)                 # tells the engine the map size the static buffers are planned for
-        N = cfg.spatial_tokens
-    else:
-        N = (batch["points"] if cfg.tokenizer == "keypoint" else batch["boxes"]).shape[1]
-    path = os.path.join(str(tmp_path), f"{name}.glgplan")
-    info = export_plan(eng, 2 * B, N, ctx.shape[1], path)
-    plan = NativePlan(path)
-    # inputs, laid out exactly as Engine._forward_cfg_rows stages them: rows [0, B) cond, rows [B, 2B) uncond / null grounding
-    plan.write("in:x", torch.cat([x, x]))
-    plan.write("in:t", torch.cat([ts, ts]))
-    plan.write("in:context", torch.cat([ctx, uc]))
-    if cfg.inpaint_mode:
-        plan.write("in:extra", torch.cat([extra, extra]))
-    z = lambda t: torch.cat([t, torch.zeros_like(t)])
-    if cfg.spatial:
-        plan.write("in:map", z(gmap)); plan.write("in:gmask", z(batch["mask"]))
-        plan.write("in:extra_map", torch.cat([gmap, gmap]))              # the uncond rows keep grounding_extra_input (plms.py:118)
-    elif cfg.tokenizer == "keypoint":
-        plan.write("in:coords", z(batch["points"])); plan.write("in:masks", z(batch["masks"]))
-    else:
-        plan.write("in:coords", z(batch["boxes"])); plan.write("in:masks", z(batch["masks"]))
-        if cfg.tokenizer == "text":
-            plan.write("in:feat0", z(batch["text_embeddings"])); plan.write("in:fmask0", z(batch["masks"]))
-        else:
-            plan.write("in:feat0", z(batch["text_embeddings"])); plan.write("in:fmask0", z(batch["text_masks"]))
-            plan.write("in:feat1", z(batch["image_embeddings"])); plan.write("in:fmask1", z(batch["image_masks"]))
-    for scale in scales:
-        set_alpha_scale(model, scale)
-        e_c, e_u = model.forward_cfg(dict(x=x, timesteps=ts, context=ctx, grounding_input=grounding, inpainting_extra_input=extra,
-                                          grounding_extra_input=gextra), uc)
-        want = torch.cat([e_c, e_u]).clone()
-        plan.write("W:gates", eng.W["gates"])                  # scale * tanh(alpha): the host owns the scheduled-sampling scale
-        plan.run(static_part=True, fuser_on=scale != 0.0)
-        plan.run(static_part=False, fuser_on=scale != 0.0)
-        got = plan.read("out", want.shape)
-        torch.cuda.synchronize()
-        assert torch.equal(got, want), f"{name} scale={scale}: max diff {(got - want).abs().max().item():.3e}"
-    plan.close()
-    return info
 
 
 @pytest.mark.parametrize("name,max_objs", [("tiny", 6), ("tiny_text_image", 5), ("tiny_keypoint", 34), ("tiny_inpaint", 6), ("tiny_sem", 0), ("tiny_hed", 0)])
