@@ -7,7 +7,8 @@
     needs `clip` / `omegaconf` to import (absent offline);
   * `sampler_inputs(...)`: the `input` dict / mask / x0 of `run()` (:384-430) from synthetic embeddings;
   * `prepare_batch(meta, batch, max_objs, encoder)` (:146-187): the box + text + image grounding batch, CLIP features from
-    gligen_b200.clip_grounding.ClipGroundingEncoder.
+    gligen_b200.clip_grounding.ClipGroundingEncoder;
+  * `sample_hires(...)`: two-pass high-resolution sampling (sample, upscale the latent, image-to-image at the target size).
 
 Shared by bench.py, __graft_entry__.smoke() and the GPU parity tests, so the benchmark never imports the test tree.
 """
@@ -170,3 +171,39 @@ def prepare_batch(meta, batch: int = 1, max_objs: int = 30, encoder=None) -> Dic
            "text_embeddings": text_embeddings.unsqueeze(0).repeat(batch, 1, 1),
            "image_embeddings": image_embeddings.unsqueeze(0).repeat(batch, 1, 1)}
     return {k: v.to(dev) for k, v in out.items()}
+
+
+def upscale_latent(z: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """Bicubic resampling (A = -0.75, align_corners = False, as F.interpolate) of an NCHW latent to H x W, in fp32 by
+    glg_resize_plane."""
+    if z.device.type != "cuda":
+        raise RuntimeError("gligen_b200 upscales latents on CUDA tensors only (no CPU fallback)")
+    from . import lib as L
+    z = z.contiguous().float()
+    B, C, Hs, Ws = z.shape
+    out = torch.empty(B, C, H, W, device=z.device, dtype=torch.float32)
+    L.check(L.load().glg_resize_plane(z.data_ptr(), z.stride(0), out.data_ptr(), B, C, Hs, Ws, H, W, 1,
+                                      torch.cuda.current_stream(z.device).cuda_stream), "glg_resize_plane")
+    return out
+
+
+def sample_hires(sampler, S, shape, input, uc, guidance_scale, scale=2, strength=0.5, S2=None):
+    """Two-pass high-resolution sampling: `sampler.sample(S, shape, ...)`, the latent upscaled by `scale` (bicubic,
+    upscale_latent), then `sampler.sample(S2 or S, upscaled shape, ..., init_latent=upscaled, strength=strength)` with the same
+    grounding `input` and `uc`.  GLIGEN's boxes are normalised, so the grounding applies unchanged to the second pass.
+    Returns the final latent at the upscaled size.
+
+    The upscaled sides must be multiples of 8.  Generator draws: pass 1's (x_T when input['x'] is None), then pass 2's start
+    noise randn(upscaled shape).  Inpainting models are refused: their inpainting_extra_input is sized for pass 1."""
+    if getattr(sampler.model, "inpaint_mode", False):
+        raise ValueError("sample_hires does not support inpainting models: their inpainting_extra_input (masked image and mask) "
+                         "has the first pass's size")
+    if not 0.0 <= strength <= 1.0:
+        raise ValueError(f"strength must lie in [0, 1], got {strength!r}")
+    B, C, H, W = shape
+    H2, W2 = int(round(H * scale)), int(round(W * scale))
+    if H2 <= 0 or W2 <= 0 or H2 % 8 or W2 % 8:
+        raise ValueError(f"latent {H}x{W} upscaled by {scale} is {H2}x{W2}: both sides must be positive multiples of 8")
+    lat = sampler.sample(S, shape, input, uc, guidance_scale)
+    up = upscale_latent(lat, H2, W2)
+    return sampler.sample(S2 or S, (B, C, H2, W2), input, uc, guidance_scale, init_latent=up, strength=strength)

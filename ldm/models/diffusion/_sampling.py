@@ -52,18 +52,48 @@ class SamplerBase(object):
         self._alphas_host = [float(v) for v in np.asarray(al, dtype=np.float64)]
         self._alphas_prev_host = [float(v) for v in np.asarray(alp, dtype=np.float64)]
 
-    # ---- pieces shared by both loops -----------------------------------------------------------
-    def _begin(self, shape, input):
-        img = input["x"]
-        if img is None:
-            img = torch.randn(shape, device=self.device)          # RNG draw #1 (plms.py:72)
+    # ---- pieces shared by every loop -----------------------------------------------------------
+    def _begin(self, shape, input, init_latent=None, strength=1.0, noise=None):
+        """(start state, the time steps to run, the scheduled-sampling alphas | None).
+
+        Without init_latent the run starts at x_T: input['x'], or randn(shape) drawn here when it is None, and covers the
+        whole grid.  With init_latent (image-to-image) it starts part-way down the grid of L = len(np.flip(ddim_timesteps))
+        steps: it runs the last n = min(L, int(strength * L)) of them, from t0 = time_range[L - n], at
+        x = sqrt(abar_t0) init_latent + sqrt(1 - abar_t0) noise (diffusion.q_sample).  input['x'] is not read; noise is the
+        caller's, or one randn(shape) drawn here, where the x_T draw would be.  n = 0 (strength 0, or strength * L < 1)
+        draws nothing and returns init_latent in fp32 with an empty step list: the caller runs no UNet pass.  The
+        scheduled-sampling alphas are alpha_generator_func(n), over the steps actually run."""
+        if init_latent is None:
+            if noise is not None or strength != 1.0:
+                raise ValueError("strength and noise apply to image-to-image only: pass init_latent as well")
+            img = input["x"]
+            if img is None:
+                img = torch.randn(shape, device=self.device)          # RNG draw #1 (plms.py:72)
+                input["x"] = img
+            time_range = np.flip(self.ddim_timesteps)
+        else:
+            if not 0.0 <= strength <= 1.0:
+                raise ValueError(f"strength must lie in [0, 1], got {strength!r}")
+            if tuple(init_latent.shape) != tuple(shape):
+                raise ValueError(f"init_latent has shape {tuple(init_latent.shape)}, the sampler was asked for {tuple(shape)}")
+            if noise is not None and tuple(noise.shape) != tuple(shape):
+                raise ValueError(f"noise has shape {tuple(noise.shape)}, the sampler was asked for {tuple(shape)}")
+            full = np.flip(self.ddim_timesteps)
+            n = min(len(full), int(strength * len(full)))
+            time_range = full[len(full) - n:]
+            init_latent = init_latent.to(self.device, torch.float32)
+            if n == 0:
+                return init_latent, time_range, None
+            if noise is None:
+                noise = torch.randn(shape, device=self.device)        # where x_T would be drawn
+            t0 = torch.full((shape[0],), int(time_range[0]), device=self.device, dtype=torch.long)
+            img = self.diffusion.q_sample(init_latent, t0, noise=noise.to(self.device, torch.float32))
             input["x"] = img
         # a new sample() call: the engine's cache of timestep-invariant work (PositionNet tokens, text K/V, grounding
         # K/V) is only an intra-loop optimisation - never trust tensor identity across calls
         inv = getattr(self.model, "invalidate_static", None)
         if inv is not None:
             inv()
-        time_range = np.flip(self.ddim_timesteps)
         alphas = self.alpha_generator_func(len(time_range)) if self.alpha_generator_func is not None else None
         return img, time_range, alphas
 

@@ -6,15 +6,17 @@ from ._sampling import SamplerBase
 
 class DDIMSampler(SamplerBase):
     @torch.no_grad()
-    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None):
+    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
+        """init_latent / strength / noise: image-to-image, started part-way down the grid (SamplerBase._begin)."""
         self.make_schedule(ddim_num_steps=S)
-        return self.ddim_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0)
+        return self.ddim_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, init_latent=init_latent, strength=strength,
+                                  noise=noise)
 
     @torch.no_grad()
-    def ddim_sampling(self, shape, input, uc, guidance_scale=1, mask=None, x0=None):
+    def ddim_sampling(self, shape, input, uc, guidance_scale=1, mask=None, x0=None, init_latent=None, strength=1.0, noise=None):
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input)
-        total = self.ddim_timesteps.shape[0]
+        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
+        total = len(time_range)                                 # step i runs at ddim_timesteps[total - i - 1]
         for i, step in enumerate(time_range):
             self._apply_alpha(alphas, i)
             index = total - i - 1

@@ -8,15 +8,18 @@ from ._sampling import AB_COEFS, SamplerBase
 
 class PLMSSampler(SamplerBase):
     @torch.no_grad()
-    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None):
+    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
+        """init_latent / strength / noise: image-to-image, started part-way down the grid (SamplerBase._begin).  The first
+        step is the pseudo improved Euler step, so a run of n steps takes n + 1 UNet passes."""
         self.make_schedule(ddim_num_steps=S)
-        return self.plms_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0)
+        return self.plms_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, init_latent=init_latent, strength=strength,
+                                  noise=noise)
 
     @torch.no_grad()
-    def plms_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None):
+    def plms_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, init_latent=None, strength=1.0, noise=None):
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input)
-        total = self.ddim_timesteps.shape[0]
+        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
+        total = len(time_range)                                 # step i runs at ddim_timesteps[total - i - 1]
         history = []                                            # newest first: e_{t-1}, e_{t-2}, e_{t-3}
         for i, step in enumerate(time_range):
             self._apply_alpha(alphas, i)

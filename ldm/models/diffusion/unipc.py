@@ -110,7 +110,8 @@ def unipc_solve(x, alpha, sigma, order, model_fn, update_fn):
 
 class UniPCSampler(SamplerBase):
     """Generator draws: randn(shape) for x_T when input['x'] is None, and one randn_like per step for the q_sample noise of the
-    inpainting blend when a mask is given.  Nothing else, as DPMSolverSampler."""
+    inpainting blend when a mask is given.  With init_latent, randn(shape) for the noise of the start state in place of x_T, none
+    when the caller passes noise or no step runs.  Nothing else, as DPMSolverSampler."""
 
     def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2):
         if order not in (1, 2, 3):
@@ -119,14 +120,19 @@ class UniPCSampler(SamplerBase):
         self.order = order
 
     @torch.no_grad()
-    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None):
+    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
+        """init_latent / strength / noise: image-to-image, started part-way down the grid (SamplerBase._begin).  The (alpha,
+        sigma) grid is the truncated time steps plus alphas_cumprod[0]; step_orders lowers the orders at its start as usual."""
         self.make_schedule(ddim_num_steps=S)
-        return self.unipc_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0)
+        return self.unipc_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, init_latent=init_latent, strength=strength,
+                                   noise=noise)
 
     @torch.no_grad()
-    def unipc_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None):
+    def unipc_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, init_latent=None, strength=1.0, noise=None):
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input)
+        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
+        if len(time_range) == 0:                                # strength 0: init_latent as it is
+            return img
         alpha, sigma = grid_alpha_sigma(self.diffusion.alphas_cumprod, time_range)
 
         def model_fn(i, x):
