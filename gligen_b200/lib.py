@@ -87,6 +87,8 @@ SIGNATURES = {
                                c_float, c_float, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_int64, c_void_p]),
     "glg_unipc_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_float, c_float]
                          + [c_float] * 9 + [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "glg_sde_update": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p]
+                       + [c_float] * 7 + [c_void_p, c_void_p, c_int64, c_void_p]),
 }
 # not part of the public header: test hook
 _DEBUG_SIGNATURES = {"glg_debug_force_bn": (None, [c_int]), "glg_debug_pick_tile": (None, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64, C.POINTER(c_int)]), "glg_debug_attn_mode": (None, [c_int]), "glg_debug_attn_poly_share": (None, [c_int]), "glg_debug_gemm_cta2": (None, [c_int]), "glg_debug_splitk": (None, [c_int]), "glg_debug_gemm_bres": (None, [c_int]), "glg_debug_gemm_pp": (None, [c_int]), "glg_debug_pick_pingpong": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64]), "glg_debug_epilogue_kind": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_int])}

@@ -400,6 +400,18 @@ class CudaOps:
                 "glg_dpm_update")
         self._note("dpm_update")
 
+    def sde_update(self, x, e_cond, e_uncond, guidance, m1, z, alpha, sigma, coefs, x0_out, x_next):
+        """One stochastic step (glg_sde_update): x0_out = (x - sigma e) / alpha, x_next = cx x + k0 x0_out + k1 m1 + ce e + cz z
+        with coefs = (cx, k0, k1, ce, cz); e the CFG mix of e_cond / e_uncond; m1 and x0_out may be None.  Outputs alias no input."""
+        assert len(coefs) == 5
+        for t in (x, e_cond, e_uncond, m1, z, x0_out, x_next):
+            assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == x.numel())
+        L.check(self._c.glg_sde_update(x.data_ptr(), e_cond.data_ptr(), _ptr(e_uncond), float(guidance), _ptr(m1), z.data_ptr(),
+                                        float(alpha), float(sigma), *(float(c) for c in coefs), _ptr(x0_out), x_next.data_ptr(),
+                                        x.numel(), self._stream()),
+                "glg_sde_update")
+        self._note("sde_update")
+
     def unipc_update(self, x, xc_prev, e_cond, e_uncond, guidance, m1, m2, m3, alpha, sigma, coefs, m_out, xc_out, x_next):
         """One UniPC step (glg_unipc_update): m_out = (x - sigma e) / alpha, xc_out = cc xc_prev + c0 m_out + c1 m1 + c2 m2 + c3 m3
         (xc_out = x when xc_prev is None), x_next = pc xc_out + p0 m_out + p1 m1 + p2 m2 with coefs = (cc, c0, c1, c2, c3, pc, p0,

@@ -285,6 +285,22 @@ int glg_unipc_update(const float* x, const float* xc_prev, const float* e_cond, 
                      float cc, float c0, float c1, float c2, float c3, float pc, float p0, float p1, float p2,
                      float* m_out, float* xc_out, float* x_next, int64_t n, void* stream);
 
+/* ---- stochastic sampler update (DDIM with eta > 0, DPM-Solver++ 2M SDE), one fused fp32 kernel ------------------------------
+ * e      = e_u + g*(e_c - e_u)                       (if e_uncond != NULL, else e = e_cond)
+ * x0_out = m0 = (x - sigma*e) / alpha                 data prediction at the evaluated timestep s (x0_out nullable: not stored)
+ * x_next = cx*x + k0*m0 + k1*m1 + ce*e + cz*z         (m1 nullable, read as 0: the previous data prediction; z required: N(0, 1))
+ * alpha = sqrt(ac_s), sigma = sqrt(1 - ac_s).  The host expands each step into (cx, k0, k1, ce, cz) in float64 (passed as fp32):
+ *   DDIM (ddim.py p_sample_ddim), a = ac_s, a' = ac_t, sigma_t = eta sqrt((1 - a')/(1 - a)) sqrt(1 - a/a'):
+ *       cx = 0, k0 = sqrt(a'), k1 = 0, ce = sqrt(1 - a' - sigma_t^2), cz = sigma_t
+ *   DPM-Solver++ 2M SDE (midpoint), lambda = log(alpha/sigma), h = lambda_t - lambda_s, r = (lambda_s - lambda_{s-1})/h,
+ *   E = -expm1(-(1 + eta) h):
+ *       cx = (sigma_t/sigma_s) exp(-eta h), k0 = alpha_t E (1 + 1/(2r)), k1 = -alpha_t E/(2r), ce = 0,
+ *       cz = sigma_t sqrt(-expm1(-2 eta h))                                  (order 1: k0 = alpha_t E, k1 = 0)
+ * The outputs must not alias any input or each other.  Any n >= 0; 16-byte-aligned pointers take 16-byte accesses. */
+int glg_sde_update(const float* x, const float* e_cond, const float* e_uncond, float guidance, const float* m1, const float* z,
+                   float alpha, float sigma, float cx, float k0, float k1, float ce, float cz, float* x0_out, float* x_next, int64_t n,
+                   void* stream);
+
 /* ---- engine level: a whole UNet forward from an exported plan ----------------------------------
  * Replaces UNetModel.forward (openaimodel.py:420-464) for hosts that cannot embed Python.  gligen_b200/export.py writes one
  * (batch rows, grounding slots, context length) plan of the engine to a file: packed weights, workspace sizes and the ordered

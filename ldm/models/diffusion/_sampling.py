@@ -29,8 +29,10 @@ class SamplerBase(object):
         setattr(self, name, attr)
 
     def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=False):
-        if ddim_eta != 0:
-            raise ValueError("ddim_eta must be 0 (the fused update has no noise term)")
+        """ddim_eta in [0, 1]: the DDIM noise scale (0 deterministic, 1 the DDPM posterior variance); DDIMSampler reads it."""
+        if not 0.0 <= ddim_eta <= 1.0:
+            raise ValueError(f"ddim_eta must lie in [0, 1], got {ddim_eta!r}")
+        self.ddim_eta = float(ddim_eta)
         self.ddim_timesteps = make_ddim_timesteps(ddim_discr_method=ddim_discretize, num_ddim_timesteps=ddim_num_steps,
                                                   num_ddpm_timesteps=self.ddpm_num_timesteps, verbose=verbose)
         ac = self.diffusion.alphas_cumprod
@@ -51,6 +53,7 @@ class SamplerBase(object):
         # pass every step (float(tensor[i]) is a device-to-host sync)
         self._alphas_host = [float(v) for v in np.asarray(al, dtype=np.float64)]
         self._alphas_prev_host = [float(v) for v in np.asarray(alp, dtype=np.float64)]
+        self._sigmas_host = [float(v) for v in np.asarray(sig, dtype=np.float64)]
 
     # ---- pieces shared by every loop -----------------------------------------------------------
     def _begin(self, shape, input, init_latent=None, strength=1.0, noise=None):
@@ -135,6 +138,25 @@ class SamplerBase(object):
                                         None if e_out is None else e_out.data_ptr(), x_prev.data_ptr(), x.numel(), st),
                   "glg_sampler_update")
         return x_prev, e_out
+
+    def _sde_update(self, x, e_c, e_u, guidance_scale, m1, z, alpha, sigma, coefs, m0_out):
+        """Fused CFG mix + data prediction (into m0_out | None) + stochastic update (glg_sde_update) with coefs = (cx, k0, k1,
+        ce, cz) and the caller's standard normal z.  Returns x at the next grid point."""
+        if x.device.type != "cuda":
+            raise RuntimeError("gligen_b200 samplers run on CUDA tensors only (no CPU fallback)")
+        x = x.contiguous().float()
+        e_c = e_c.contiguous().float()
+        e_u = None if e_u is None else e_u.contiguous().float()
+        z = z.contiguous().float()
+        x_next = torch.empty_like(x)
+        lib = _L.load()
+        st = torch.cuda.current_stream(x.device).cuda_stream
+        ptr = lambda t: None if t is None else t.data_ptr()
+        _L.check(lib.glg_sde_update(x.data_ptr(), e_c.data_ptr(), ptr(e_u), float(guidance_scale), ptr(m1), z.data_ptr(),
+                                    float(alpha), float(sigma), *(float(c) for c in coefs), ptr(m0_out), x_next.data_ptr(),
+                                    x.numel(), st),
+                 "glg_sde_update")
+        return x_next
 
     def _inpaint_blend(self, img, mask, x0, ts):
         if mask is None:

@@ -67,6 +67,45 @@ def grid_alpha_sigma(alphas_cumprod, time_range):
     return np.sqrt(grid), np.sqrt(1.0 - grid)
 
 
+def sde_coefficients(alpha, sigma, orders, eta):
+    """float64 [n, 5]: (cx, k0, k1, ce, cz) of the DPM-Solver++ 2M SDE step (midpoint form) x_next = cx x + k0 m0 + k1 m1 + cz z,
+    ce = 0, for each step of order 1 or 2; alpha, sigma as for step_coefficients.  With h = lambda_t - lambda_s, r = h_prev / h and
+    E = -expm1(-(1 + eta) h): cx = (sigma_t / sigma_s) exp(-eta h), k0 = alpha_t E (1 + 1 / (2 r)), k1 = -alpha_t E / (2 r),
+    cz = sigma_t sqrt(-expm1(-2 eta h)); order 1 drops the r terms.  eta = 0 gives step_coefficients' (cx, k0, k1)."""
+    alpha = np.asarray(alpha, dtype=np.float64)
+    sigma = np.asarray(sigma, dtype=np.float64)
+    lam = np.log(alpha) - np.log(sigma)
+    out = np.zeros((len(orders), 5))
+    for i, k in enumerate(orders):
+        if k not in (1, 2):
+            raise ValueError(f"the SDE step has orders 1 and 2, got {k!r}")
+        h = lam[i + 1] - lam[i]
+        big_e = -np.expm1(-(1.0 + eta) * h)
+        a_t, s_t = alpha[i + 1], sigma[i + 1]
+        out[i, 0] = s_t / sigma[i] * np.exp(-eta * h)
+        out[i, 1] = a_t * big_e
+        if k == 2:
+            r = (lam[i] - lam[i - 1]) / h
+            out[i, 1] += a_t * big_e / (2.0 * r)
+            out[i, 2] = -a_t * big_e / (2.0 * r)
+        out[i, 4] = s_t * np.sqrt(-np.expm1(-2.0 * eta * h))
+    return out
+
+
+def sde_solve(x, alpha, sigma, order, eta, model_fn, update_fn):
+    """The 2M SDE loop over the n + 1 grid points of (alpha, sigma), orders from step_orders.  model_fn as for dpm_solve;
+    update_fn(x, e_cond, e_uncond, m1, alpha_i, sigma_i, coefs, m0_out) -> x at point i + 1 (it draws the step's noise).  The data
+    predictions rotate through two buffers allocated once."""
+    orders = step_orders(len(alpha) - 1, order)
+    coefs = sde_coefficients(alpha, sigma, orders, eta)
+    hist = [torch.empty_like(x) for _ in range(2)]
+    for i, k in enumerate(orders):
+        x, e_c, e_u = model_fn(i, x)
+        m1 = hist[(i - 1) % 2] if k >= 2 else None
+        x = update_fn(x, e_c, e_u, m1, float(alpha[i]), float(sigma[i]), [float(c) for c in coefs[i]], hist[i % 2])
+    return x
+
+
 def dpm_solve(x, alpha, sigma, order, model_fn, update_fn):
     """The multistep loop over the n + 1 grid points of (alpha, sigma).  model_fn(i, x) -> (x, e_cond, e_uncond | None): the
     model at grid point i (it may replace x, as the inpainting blend does).  update_fn(x, e_cond, e_uncond, m1, m2, alpha_i,
@@ -87,13 +126,21 @@ class DPMSolverSampler(SamplerBase):
     """Generator draws: randn(shape) for x_T when input['x'] is None, and one randn_like per step for the q_sample noise of the
     inpainting blend when a mask is given.  With init_latent, randn(shape) for the noise of the start state in place of x_T, none
     when the caller passes noise or no step runs.  Nothing else: unlike PLMSSampler and DDIMSampler there is no dropped sigma = 0 draw
-    per step, so a run with the same seed consumes a different stream from theirs."""
+    per step, so a run with the same seed consumes a different stream from theirs.
 
-    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2):
+    eta > 0 (orders 1 and 2) is DPM-Solver++ 2M SDE (sde_coefficients, one glg_sde_update per step): it also draws one
+    randn_like(x) per step after the model pass, the last step included, after the blend's draw when there is a mask."""
+
+    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2, eta=0.0):
         if order not in (1, 2, 3):
             raise ValueError(f"DPM-Solver++ order must be 1, 2 or 3, got {order!r}")
+        if not 0.0 <= eta <= 1.0:
+            raise ValueError(f"eta must lie in [0, 1], got {eta!r}")
+        if eta > 0 and order == 3:
+            raise ValueError("the SDE form (eta > 0) has orders 1 and 2 only")
         super().__init__(diffusion, model, schedule, alpha_generator_func, set_alpha_scale)
         self.order = order
+        self.eta = float(eta)
 
     @torch.no_grad()
     def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
@@ -124,6 +171,14 @@ class DPMSolverSampler(SamplerBase):
             input["x"] = x
             return x
 
+        if self.eta > 0:
+            def sde_fn(x, e_c, e_u, m1, a, s, coefs, m0_out):
+                z = torch.randn_like(x)
+                x = self._sde_update(x, e_c, e_u, guidance_scale, m1, z, a, s, coefs, m0_out)
+                input["x"] = x
+                return x
+
+            return sde_solve(img.contiguous().float(), alpha, sigma, self.order, self.eta, model_fn, sde_fn)
         return dpm_solve(img.contiguous().float(), alpha, sigma, self.order, model_fn, update_fn)
 
     def _dpm_update(self, x, e_c, e_u, guidance_scale, m1, m2, alpha, sigma, coefs, m0_out):

@@ -7,6 +7,11 @@ from ._sampling import AB_COEFS, SamplerBase
 
 
 class PLMSSampler(SamplerBase):
+    def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=False):
+        if ddim_eta != 0:
+            raise ValueError("ddim_eta must be 0 for PLMS")            # as the reference's (plms.py:25-27)
+        super().make_schedule(ddim_num_steps, ddim_discretize, ddim_eta, verbose)
+
     @torch.no_grad()
     def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
         """init_latent / strength / noise: image-to-image, started part-way down the grid (SamplerBase._begin).  The first
