@@ -274,7 +274,10 @@ __global__ void copy_rows_kernel(const bf16* __restrict__ x, long long ldx, bf16
   }
 }
 
-__global__ void timestep_embedding_kernel(const long long* __restrict__ t, bf16* __restrict__ out, int B, int dim) {
+// T = long long (integer grid timesteps) or float (fractional model time); util.py:170 evaluates timesteps.float() * freqs, so both
+// round t to fp32 first and share every instruction after that: integer-valued t gives the same bits through either entry point
+template <typename T>
+__global__ void timestep_embedding_kernel(const T* __restrict__ t, bf16* __restrict__ out, int B, int dim) {
   pdl_trigger();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -624,9 +627,16 @@ extern "C" int glg_copy_rows(const void* x, int64_t ldx, void* y, int64_t ldy, i
 
 extern "C" int glg_timestep_embedding(const int64_t* t, void* out, int32_t B, int32_t dim, void* stream) {
   if (dim % 2) return set_error("glg_timestep_embedding: dim must be even");
-  launch_k(timestep_embedding_kernel, dim3(blocks_for((long long)B * dim, 256)), dim3(256), 0, ST, 1, (const long long*)t, (bf16*)out, B, dim);
+  launch_k(timestep_embedding_kernel<long long>, dim3(blocks_for((long long)B * dim, 256)), dim3(256), 0, ST, 1, (const long long*)t, (bf16*)out, B, dim);
   count_launch();
   return check_launch("timestep_embedding launch");
+}
+
+extern "C" int glg_timestep_embedding_f32(const float* t, void* out, int32_t B, int32_t dim, void* stream) {
+  if (dim % 2) return set_error("glg_timestep_embedding_f32: dim must be even");
+  launch_k(timestep_embedding_kernel<float>, dim3(blocks_for((long long)B * dim, 256)), dim3(256), 0, ST, 1, t, (bf16*)out, B, dim);
+  count_launch();
+  return check_launch("timestep_embedding_f32 launch");
 }
 
 extern "C" int glg_position_features(const float* feat, int64_t feat_batch_stride, const float* feat_mask, const float* null_feat,

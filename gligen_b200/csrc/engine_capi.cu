@@ -104,6 +104,7 @@ const OpDef kOps[] = {
     {"glg_im2col_s2", "PIPIIIIT", 0, CALL(glg_im2col_s2(A_P(0), A_I(1), A_P(2), A_I32(3), A_I32(4), A_I32(5), A_I32(6), st))},
     {"glg_im2col_s2_pad", "PIPIIIIIT", 0, CALL(glg_im2col_s2_pad(A_P(0), A_I(1), A_P(2), A_I32(3), A_I32(4), A_I32(5), A_I32(6), A_I32(7), st))},
     {"glg_timestep_embedding", "PPIIT", 0, CALL(glg_timestep_embedding((const int64_t*)A_P(0), A_P(1), A_I32(2), A_I32(3), st))},
+    {"glg_timestep_embedding_f32", "PPIIT", 0, CALL(glg_timestep_embedding_f32((const float*)A_P(0), A_P(1), A_I32(2), A_I32(3), st))},
     {"glg_position_features", "PIPPPPPPIIIIIIT", 0,
      CALL(glg_position_features((const float*)A_P(0), A_I(1), (const float*)A_P(2), (const float*)A_P(3), (const float*)A_P(4),
                                 (const float*)A_P(5), (const float*)A_P(6), A_P(7), A_I(8), A_I32(9), A_I32(10), A_I32(11), A_I32(12),

@@ -56,7 +56,7 @@ class Engine(EngineBase):
         self.cfg = cfg
         self.blocks = block_schedule(cfg)
         self.W: Dict[str, torch.Tensor] = {}
-        self.plans: Dict[Tuple[int, ...], Plan] = {}
+        self.plans: Dict[tuple, Plan] = {}
         self.scale = 1.0
         self.use_graphs = use_graphs and self.dev.type == "cuda"
         self.loaded = False
@@ -306,8 +306,9 @@ class Engine(EngineBase):
                     s["up"] = max(s["up"], Bt * hw * 4 * ly.cin)
         return s
 
-    def _build_plan(self, Bt: int, N: int, nctx: int, Hl: int, Wl: int) -> Plan:
-        """Plan for a [Bt, in_channels, Hl, Wl] latent."""
+    def _build_plan(self, Bt: int, N: int, nctx: int, Hl: int, Wl: int, fractional_t: bool = False) -> Plan:
+        """Plan for a [Bt, in_channels, Hl, Wl] latent.  fractional_t: the timestep input is fp32 (model time between the integer
+        DDPM steps) and the embedding step runs glg_timestep_embedding_f32; otherwise it is int64."""
         cfg, ops, W = self.cfg, self.ops, self.W
         S = self.n_streams
         G = N * S
@@ -329,7 +330,7 @@ class Engine(EngineBase):
         P.inp["x"] = self._zeros(Bt, cfg.in_channels, Hl, Wl)
         if cfg.inpaint_mode:
             P.inp["extra"] = self._zeros(Bt, cfg.in_channels + 1, Hl, Wl)
-        P.inp["t"] = self._zeros(Bt, dtype=torch.int64)
+        P.inp["t"] = self._zeros(Bt, dtype=torch.float32 if fractional_t else torch.int64)
         P.inp["context"] = self._zeros(Bt, nctx, cfg.context_dim)
         if cfg.spatial:
             P.inp["map"] = self._zeros(Bt, *self._map_shape)          # the conditioning map (null rows: zeros)
@@ -605,8 +606,10 @@ class Engine(EngineBase):
     # ------------------------------------------------------------------------------------------
     # execution
     # ------------------------------------------------------------------------------------------
-    def _plan(self, Bt: int, N: int, nctx: int, slot: int = 0, H: Optional[int] = None, W: Optional[int] = None) -> Plan:
-        """Plan for Bt rows of an H x W latent (default: cfg.image_size square)."""
+    def _plan(self, Bt: int, N: int, nctx: int, slot: int = 0, H: Optional[int] = None, W: Optional[int] = None,
+              fractional_t: bool = False) -> Plan:
+        """Plan for Bt rows of an H x W latent (default: cfg.image_size square), taking int64 timesteps, or fp32 ones with
+        fractional_t (a plan of its own, built only when a caller passes floating timesteps)."""
         H = self.cfg.image_size if H is None else H
         W = self.cfg.image_size if W is None else W
         self.check_latent_size(H, W)
@@ -615,9 +618,9 @@ class Engine(EngineBase):
             raise AssertionError("Grounding tokens must be square rootable")     # the reference's assert (attention.py:278)
         # one plan (and static-part cache) per latent size and batch chunk; the square default size keeps the short key
         size = () if H == W == self.cfg.image_size else (H, W)
-        key = (Bt, N, nctx) + size + ((slot,) if slot else ())
+        key = (Bt, N, nctx) + size + ((slot,) if slot else ()) + (("f32_t",) if fractional_t else ())
         if key not in self.plans:
-            self.plans[key] = self._build_plan(Bt, N, nctx, H, W)
+            self.plans[key] = self._build_plan(Bt, N, nctx, H, W, fractional_t)
         return self.plans[key]
 
     def check_latent_size(self, H: int, W: int) -> None:
@@ -744,6 +747,14 @@ class Engine(EngineBase):
     MAX_ROWS = 64
 
     @staticmethod
+    def _timesteps(timesteps):
+        """(timesteps as the plan's t input takes them, fractional?).  Floating timesteps may be fractional (util.py:160-180) and
+        run the fp32-t plan, converted to fp32 as the reference's timesteps.float() does; integer ones run the int64 plan."""
+        if timesteps.is_floating_point():
+            return timesteps.float(), True
+        return timesteps, False
+
+    @staticmethod
     def _rows(t, lo, hi):
         if t is None:
             return None
@@ -783,7 +794,8 @@ class Engine(EngineBase):
                                "of the last prepared one (GroundingNetInput.get_null_input asserts the same)")
         else:
             N = self._last_N
-        P = self._plan(B, N, context.shape[1], slot, *x.shape[2:])
+        timesteps, frac = self._timesteps(timesteps)
+        P = self._plan(B, N, context.shape[1], slot, *x.shape[2:], fractional_t=frac)
         P.inp["x"].copy_(x)
         P.inp["t"].copy_(timesteps)
         if self.cfg.inpaint_mode:
@@ -818,7 +830,8 @@ class Engine(EngineBase):
         B = x.shape[0]
         N = self._n_objs(grounding)
         self._last_N = N
-        P = self._plan(2 * B, N, context.shape[1], slot, *x.shape[2:])
+        timesteps, frac = self._timesteps(timesteps)
+        P = self._plan(2 * B, N, context.shape[1], slot, *x.shape[2:], fractional_t=frac)
         P.inp["x"][:B].copy_(x); P.inp["x"][B:].copy_(x)
         P.inp["t"][:B].copy_(timesteps); P.inp["t"][B:].copy_(timesteps)
         if self.cfg.inpaint_mode:

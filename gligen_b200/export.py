@@ -51,13 +51,16 @@ def _registry(eng, P) -> List[Tuple[str, torch.Tensor, bool]]:
     return reg
 
 
-def export_plan(eng, rows: int, n_objs: int, n_ctx: int, path: str, H: Optional[int] = None, W: Optional[int] = None) -> Dict[str, int]:
+def export_plan(eng, rows: int, n_objs: int, n_ctx: int, path: str, H: Optional[int] = None, W: Optional[int] = None,
+                fractional_t: bool = False) -> Dict[str, int]:
     """Write the plan for (rows, n_objs, n_ctx) at an H x W latent (default: the config's square size) - rows = 2B when cond +
     uncond run as one batch.  The latent size is baked into the recorded calls and the sizes of "in:x" / "out".  Returns counts.
+    "in:t" is int64 [rows], the integer DDPM steps; with fractional_t it is fp32 [rows], model time that may lie between them
+    (the continuous-time grids of the Karras samplers), embedded by glg_timestep_embedding_f32.
     Spatial-map models: n_objs = cfg.spatial_tokens, and the engine must have seen one grounded call (or `eng._n_objs(grounding)`)
     so that it knows the (C, H, W) of the conditioning map its static buffers are sized for; the named inputs are then
     "in:map", "in:gmask" and "in:extra_map"."""
-    P = eng._plan(rows, n_objs, n_ctx, H=H, W=W)
+    P = eng._plan(rows, n_objs, n_ctx, H=H, W=W, fractional_t=fractional_t)
     reg = _registry(eng, P)
     spans = []
     for bi, (name, t, _) in enumerate(reg):

@@ -57,6 +57,7 @@ SIGNATURES = {
     "glg_im2col_s2_pad": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "glg_copy_rows": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p]),
     "glg_timestep_embedding": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "glg_timestep_embedding_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "glg_position_features": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                       c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "glg_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),

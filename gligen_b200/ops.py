@@ -234,9 +234,14 @@ class CudaOps:
         self._note("im2col_s2")
 
     def timestep_embedding(self, t, out):
-        assert t.dtype == torch.int64 and out.is_contiguous()
-        L.check(self._c.glg_timestep_embedding(t.data_ptr(), out.data_ptr(), out.shape[0], out.shape[1], self._stream()),
-                "glg_timestep_embedding")
+        """t int64 (the integer DDPM steps) or fp32 (fractional model time) [B] -> out bf16 [B, dim]."""
+        assert t.dtype in (torch.int64, torch.float32) and t.is_contiguous() and out.is_contiguous()
+        if t.dtype == torch.int64:
+            L.check(self._c.glg_timestep_embedding(t.data_ptr(), out.data_ptr(), out.shape[0], out.shape[1], self._stream()),
+                    "glg_timestep_embedding")
+        else:
+            L.check(self._c.glg_timestep_embedding_f32(t.data_ptr(), out.data_ptr(), out.shape[0], out.shape[1], self._stream()),
+                    "glg_timestep_embedding_f32")
         self._note("timestep_embedding")
 
     def position_features(self, feat, feat_mask, null_feat, coords, pos_mask, null_pos, out, freqs: int):

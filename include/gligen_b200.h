@@ -159,6 +159,10 @@ int glg_im2col_s2_pad(const void* x, int64_t ldx, void* y, int32_t B, int32_t H,
 int glg_copy_rows(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int32_t C, void* stream);
 /* timestep_embedding (util.py:160-180): out bf16 [B, dim] = [cos(t f) | sin(t f)], f_k = exp(-ln(1e4) k / (dim/2)). */
 int glg_timestep_embedding(const int64_t* t, void* out, int32_t B, int32_t dim, void* stream);
+/* the same embedding of fp32 timesteps, which may be fractional (util.py:160-180: "may be fractional", timesteps.float() * freqs):
+ * the continuous-time samplers evaluate the UNet between the integer DDPM steps.  One kernel body serves both entry points, and
+ * an integer-valued t gives the same bits through either. */
+int glg_timestep_embedding_f32(const float* t, void* out, int32_t B, int32_t dim, void* stream);
 /* PositionNet input rows (text_grounding_net.py:33-45, text_image_grounding_net.py:44-60,
  * keypoint_grounding_net.py:38-55): out bf16 [B*N, F + P] = [feat*m_f + (1-m_f)*null_f | fourier(coords)*m + (1-m)*null_p]
  * feat: fp32 [B, N, F] (feat_batch_stride = 0 broadcasts one [N, F] table over the batch); coords fp32 [B, N, ncoord];

@@ -5,11 +5,38 @@ ddim.py); the per-step arithmetic (classifier-free-guidance mix, Adams-Bashforth
 update; plms.py:121-158) is ONE fused fp32 kernel (glg_sampler_update) instead of ~10 eager launches, and
 when the model is this repo's UNetModel the cond and uncond passes run as a single 2B batch.
 """
+from typing import NamedTuple
+
 import numpy as np
 import torch
 
 from gligen_b200 import lib as _L
 from ldm.modules.diffusionmodules.util import make_ddim_sampling_parameters, make_ddim_timesteps
+
+
+class SamplingGrid(NamedTuple):
+    """The points a sampling loop visits: step i evaluates the model at times[i] and moves from grid point i to i + 1.
+    times [L]: int64 DDPM steps (the DDIM uniform grid) or float64 fractional model time (the Karras grid); alpha, sigma float64
+    [L + 1]: the VP (sqrt(abar), sqrt(1 - abar)) of each point, the last one the target of the final step."""
+    times: np.ndarray
+    alpha: np.ndarray
+    sigma: np.ndarray
+
+    @property
+    def integer(self) -> bool:
+        return self.times.dtype.kind in "iu"
+
+    def last(self, n: int) -> "SamplingGrid":
+        """The last n steps."""
+        L = len(self.times)
+        return SamplingGrid(self.times[L - n:], self.alpha[L - n:], self.sigma[L - n:])
+
+
+def grid_alpha_sigma(alphas_cumprod, time_range):
+    """float64 (alpha, sigma) [n + 1] at the timesteps of time_range followed by alphas_cumprod[0] (DDIM's last alphas_prev)."""
+    ac = np.asarray(alphas_cumprod.detach().cpu(), dtype=np.float64) if torch.is_tensor(alphas_cumprod) else alphas_cumprod
+    grid = np.append(ac[np.asarray(time_range)], ac[0])
+    return np.sqrt(grid), np.sqrt(1.0 - grid)
 
 
 class SamplerBase(object):
@@ -42,6 +69,7 @@ class SamplerBase(object):
         self.register_buffer("alphas_cumprod", f32(ac))
         self.register_buffer("alphas_cumprod_prev", f32(self.diffusion.alphas_cumprod_prev))
         acc = ac.cpu()
+        self._ac_host = np.asarray(acc, dtype=np.float64)
         self.register_buffer("sqrt_alphas_cumprod", f32(np.sqrt(acc)))
         self.register_buffer("sqrt_one_minus_alphas_cumprod", f32(np.sqrt(1. - acc)))
         sig, al, alp = make_ddim_sampling_parameters(alphacums=acc, ddim_timesteps=self.ddim_timesteps, eta=ddim_eta, verbose=verbose)
@@ -56,16 +84,23 @@ class SamplerBase(object):
         self._sigmas_host = [float(v) for v in np.asarray(sig, dtype=np.float64)]
 
     # ---- pieces shared by every loop -----------------------------------------------------------
-    def _begin(self, shape, input, init_latent=None, strength=1.0, noise=None):
-        """(start state, the time steps to run, the scheduled-sampling alphas | None).
+    def ddim_grid(self) -> SamplingGrid:
+        """The DDIM uniform grid of the last make_schedule: np.flip(ddim_timesteps), then alphas_cumprod[0]."""
+        times = np.flip(self.ddim_timesteps)
+        return SamplingGrid(times, *grid_alpha_sigma(self._ac_host, times))
+
+    def _begin(self, shape, input, init_latent=None, strength=1.0, noise=None, grid=None):
+        """(start state, the SamplingGrid of the steps to run, the scheduled-sampling alphas | None).  grid: the full grid of
+        L steps (default ddim_grid()).
 
         Without init_latent the run starts at x_T: input['x'], or randn(shape) drawn here when it is None, and covers the
-        whole grid.  With init_latent (image-to-image) it starts part-way down the grid of L = len(np.flip(ddim_timesteps))
-        steps: it runs the last n = min(L, int(strength * L)) of them, from t0 = time_range[L - n], at
-        x = sqrt(abar_t0) init_latent + sqrt(1 - abar_t0) noise (diffusion.q_sample).  input['x'] is not read; noise is the
-        caller's, or one randn(shape) drawn here, where the x_T draw would be.  n = 0 (strength 0, or strength * L < 1)
-        draws nothing and returns init_latent in fp32 with an empty step list: the caller runs no UNet pass.  The
-        scheduled-sampling alphas are alpha_generator_func(n), over the steps actually run."""
+        whole grid.  With init_latent (image-to-image) it starts part-way down the grid: it runs the last n = min(L, int(strength
+        * L)) steps, from x = alpha_0 init_latent + sigma_0 noise at their first point (on the integer grid diffusion.q_sample at
+        t0 = times[L - n], as the reference forms it).  input['x'] is not read; noise is the caller's, or one randn(shape) drawn
+        here, where the x_T draw would be.  n = 0 (strength 0, or strength * L < 1) draws nothing and returns init_latent in
+        fp32 with an empty grid: the caller runs no UNet pass.  The scheduled-sampling alphas are alpha_generator_func(n), over
+        the steps actually run."""
+        grid = self.ddim_grid() if grid is None else grid
         if init_latent is None:
             if noise is not None or strength != 1.0:
                 raise ValueError("strength and noise apply to image-to-image only: pass init_latent as well")
@@ -73,7 +108,6 @@ class SamplerBase(object):
             if img is None:
                 img = torch.randn(shape, device=self.device)          # RNG draw #1 (plms.py:72)
                 input["x"] = img
-            time_range = np.flip(self.ddim_timesteps)
         else:
             if not 0.0 <= strength <= 1.0:
                 raise ValueError(f"strength must lie in [0, 1], got {strength!r}")
@@ -81,24 +115,36 @@ class SamplerBase(object):
                 raise ValueError(f"init_latent has shape {tuple(init_latent.shape)}, the sampler was asked for {tuple(shape)}")
             if noise is not None and tuple(noise.shape) != tuple(shape):
                 raise ValueError(f"noise has shape {tuple(noise.shape)}, the sampler was asked for {tuple(shape)}")
-            full = np.flip(self.ddim_timesteps)
-            n = min(len(full), int(strength * len(full)))
-            time_range = full[len(full) - n:]
+            L = len(grid.times)
+            grid = grid.last(min(L, int(strength * L)))
             init_latent = init_latent.to(self.device, torch.float32)
-            if n == 0:
-                return init_latent, time_range, None
+            if len(grid.times) == 0:
+                return init_latent, grid, None
             if noise is None:
                 noise = torch.randn(shape, device=self.device)        # where x_T would be drawn
-            t0 = torch.full((shape[0],), int(time_range[0]), device=self.device, dtype=torch.long)
-            img = self.diffusion.q_sample(init_latent, t0, noise=noise.to(self.device, torch.float32))
+            noise = noise.to(self.device, torch.float32)
+            if grid.integer:
+                t0 = torch.full((shape[0],), int(grid.times[0]), device=self.device, dtype=torch.long)
+                img = self.diffusion.q_sample(init_latent, t0, noise=noise)
+            else:
+                img = float(grid.alpha[0]) * init_latent + float(grid.sigma[0]) * noise
             input["x"] = img
         # a new sample() call: the engine's cache of timestep-invariant work (PositionNet tokens, text K/V, grounding
         # K/V) is only an intra-loop optimisation - never trust tensor identity across calls
         inv = getattr(self.model, "invalidate_static", None)
         if inv is not None:
             inv()
-        alphas = self.alpha_generator_func(len(time_range)) if self.alpha_generator_func is not None else None
-        return img, time_range, alphas
+        alphas = self.alpha_generator_func(len(grid.times)) if self.alpha_generator_func is not None else None
+        return img, grid, alphas
+
+    def _point(self, x, grid, i, b, mask, x0):
+        """(x after the inpainting blend, the timesteps tensor) of step i of grid: int64 DDPM steps on the integer grid, fp32
+        model time on a fractional one (the UNet then runs its fp32-timestep plan)."""
+        if grid.integer:
+            ts = torch.full((b,), int(grid.times[i]), device=self.device, dtype=torch.long)
+            return self._inpaint_blend(x, mask, x0, ts), ts
+        ts = torch.full((b,), float(grid.times[i]), device=self.device, dtype=torch.float32)
+        return self._inpaint_blend(x, mask, x0, ts, float(grid.alpha[i]), float(grid.sigma[i])), ts
 
     def _apply_alpha(self, alphas, i):
         if alphas is not None:
@@ -158,11 +204,15 @@ class SamplerBase(object):
                  "glg_sde_update")
         return x_next
 
-    def _inpaint_blend(self, img, mask, x0, ts):
+    def _inpaint_blend(self, img, mask, x0, ts, alpha=None, sigma=None):
+        """The inpainting mask blend at the step's point: diffusion.q_sample(x0, ts) on the integer grid (plms.py:96-100); at a
+        fractional point (alpha, sigma given) x0 alpha + sigma randn_like(x0), the same single draw as q_sample's."""
         if mask is None:
             return img
         assert x0 is not None
-        return self.diffusion.q_sample(x0, ts) * mask + (1. - mask) * img      # plms.py:96-100
+        if alpha is None:
+            return self.diffusion.q_sample(x0, ts) * mask + (1. - mask) * img      # plms.py:96-100
+        return (alpha * x0 + sigma * torch.randn_like(x0)) * mask + (1. - mask) * img
 
 
 AB_COEFS = {

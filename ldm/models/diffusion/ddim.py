@@ -31,7 +31,8 @@ class DDIMSampler(SamplerBase):
         """Runs at the eta of the last make_schedule call.  Generator draws as the reference's: x_T (SamplerBase._begin), then per
         step the inpainting blend's q_sample noise (with a mask) and one randn_like(x) after the model pass."""
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
+        img, grid, alphas = self._begin(shape, input, init_latent, strength, noise)
+        time_range = grid.times
         stochastic = self.ddim_eta > 0
         total = len(time_range)                                 # step i runs at ddim_timesteps[total - i - 1]
         for i, step in enumerate(time_range):

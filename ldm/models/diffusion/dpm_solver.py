@@ -5,7 +5,9 @@ Probabilistic Models", Algorithm 2) with PLMSSampler's call surface plus `order`
                      guidance_scale, mask, x0) -> x0 latent
 
 It steps on the DDIM uniform grid of PLMS and DDIM (S = 30 gives 31 steps; the last step goes to alphas_cumprod[0]) with one UNet
-pass per step (one 2B pass when CFG is on), so S = 20 costs 20 passes where PLMSSampler.sample(S=50) costs 51.  Scheduled
+pass per step (one 2B pass when CFG is on), so S = 20 costs 20 passes where PLMSSampler.sample(S=50) costs 51.  grid="karras" steps
+on the Karras sigma grid instead (_karras.py): exactly S steps and S passes, the UNet evaluated at fractional timesteps, the final
+step to sigma = 0 first order (x_S = m_{S-1}, k-diffusion's sample_dpmpp_2m / sample_dpmpp_2m_sde).  Scheduled
 sampling, the first-conv swap and the inpainting blend are SamplerBase's.  Order 1 is DDIM with eta = 0.  The CFG mix, the data
 prediction and the multistep update are one fp32 kernel per step (glg_dpm_update); the per-step scalars come from float64 host
 tables, so the loop never waits on the device.
@@ -15,7 +17,10 @@ import torch
 
 from gligen_b200 import lib as _L
 
-from ._sampling import SamplerBase
+from . import _karras
+from ._sampling import SamplerBase, grid_alpha_sigma  # noqa: F401  (grid_alpha_sigma: re-exported for callers of this module)
+
+GRIDS = ("ddim", "karras")
 
 # below this many steps the last step is first order and the one before at most second order (the final steps of a short run
 # are the largest in lambda, where the higher-order terms lose accuracy)
@@ -60,11 +65,35 @@ def step_coefficients(alpha, sigma, orders):
     return out
 
 
-def grid_alpha_sigma(alphas_cumprod, time_range):
-    """float64 (alpha, sigma) [n + 1] at the timesteps of time_range followed by alphas_cumprod[0] (DDIM's last alphas_prev)."""
-    ac = np.asarray(alphas_cumprod.detach().cpu(), dtype=np.float64)
-    grid = np.append(ac[np.asarray(time_range)], ac[0])
-    return np.sqrt(grid), np.sqrt(1.0 - grid)
+def grid_orders(sigma, order):
+    """step_orders over the n steps of a grid of n + 1 points; a final step to sigma = 0 is first order whatever n (its target
+    is the data prediction itself: x_S = m_{S-1})."""
+    orders = step_orders(len(sigma) - 1, order)
+    if sigma[-1] == 0.0:
+        orders[-1] = 1
+    return orders
+
+
+def _to_zero(table, alpha, sigma, orders, final_row):
+    """table(alpha, sigma, orders) with its last row replaced by final_row when the grid ends at sigma = 0 (lambda = +inf): the
+    rows before it see only the finite points, and the final row is stated, not derived through infinite arithmetic."""
+    if sigma[-1] > 0.0:
+        return table(alpha, sigma, orders)
+    out = np.zeros((len(orders), len(final_row)))
+    out[:-1] = table(alpha[:-1], sigma[:-1], orders[:-1])
+    out[-1] = final_row
+    return out
+
+
+def grid_coefficients(alpha, sigma, orders):
+    """step_coefficients, with the final step to sigma = 0 (when the grid ends there) the row x_S = m_{S-1}: (0, 1, 0, 0)."""
+    return _to_zero(step_coefficients, alpha, sigma, orders, (0.0, 1.0, 0.0, 0.0))
+
+
+def grid_sde_coefficients(alpha, sigma, orders, eta):
+    """sde_coefficients, with the final step to sigma = 0 (when the grid ends there) the noiseless row x_S = m_{S-1}:
+    (0, 1, 0, 0, 0)."""
+    return _to_zero(lambda a, s, o: sde_coefficients(a, s, o, eta), alpha, sigma, orders, (0.0, 1.0, 0.0, 0.0, 0.0))
 
 
 def sde_coefficients(alpha, sigma, orders, eta):
@@ -92,17 +121,22 @@ def sde_coefficients(alpha, sigma, orders, eta):
     return out
 
 
-def sde_solve(x, alpha, sigma, order, eta, model_fn, update_fn):
-    """The 2M SDE loop over the n + 1 grid points of (alpha, sigma), orders from step_orders.  model_fn as for dpm_solve;
-    update_fn(x, e_cond, e_uncond, m1, alpha_i, sigma_i, coefs, m0_out) -> x at point i + 1 (it draws the step's noise).  The data
-    predictions rotate through two buffers allocated once."""
-    orders = step_orders(len(alpha) - 1, order)
-    coefs = sde_coefficients(alpha, sigma, orders, eta)
+def sde_solve(x, alpha, sigma, order, eta, model_fn, update_fn, final_fn):
+    """The 2M SDE loop over the n + 1 grid points of (alpha, sigma), orders from grid_orders.  model_fn as for dpm_solve;
+    update_fn(x, e_cond, e_uncond, m1, alpha_i, sigma_i, coefs, m0_out) -> x at point i + 1 (it draws the step's noise).  A grid
+    ending at sigma = 0 ends with the noiseless step x_S = m_{S-1}: final_fn(x, e_cond, e_uncond, alpha_i, sigma_i, coefs (cx, k0,
+    k1, 0), m0_out) runs it and draws nothing.  The data predictions rotate through two buffers allocated once."""
+    orders = grid_orders(sigma, order)
+    coefs = grid_sde_coefficients(alpha, sigma, orders, eta)
     hist = [torch.empty_like(x) for _ in range(2)]
     for i, k in enumerate(orders):
         x, e_c, e_u = model_fn(i, x)
         m1 = hist[(i - 1) % 2] if k >= 2 else None
-        x = update_fn(x, e_c, e_u, m1, float(alpha[i]), float(sigma[i]), [float(c) for c in coefs[i]], hist[i % 2])
+        c = [float(v) for v in coefs[i]]
+        if sigma[i + 1] == 0.0:
+            x = final_fn(x, e_c, e_u, float(alpha[i]), float(sigma[i]), c[:3] + [0.0], hist[i % 2])
+        else:
+            x = update_fn(x, e_c, e_u, m1, float(alpha[i]), float(sigma[i]), c, hist[i % 2])
     return x
 
 
@@ -111,8 +145,8 @@ def dpm_solve(x, alpha, sigma, order, model_fn, update_fn):
     model at grid point i (it may replace x, as the inpainting blend does).  update_fn(x, e_cond, e_uncond, m1, m2, alpha_i,
     sigma_i, coefs, m0_out) -> x at point i + 1, writing this step's data prediction into m0_out.  The data predictions rotate
     through three buffers allocated once: step i writes buffer i % 3 and reads the two before it."""
-    orders = step_orders(len(alpha) - 1, order)
-    coefs = step_coefficients(alpha, sigma, orders)
+    orders = grid_orders(sigma, order)
+    coefs = grid_coefficients(alpha, sigma, orders)
     hist = [torch.empty_like(x) for _ in range(3)]
     for i, k in enumerate(orders):
         x, e_c, e_u = model_fn(i, x)
@@ -129,11 +163,18 @@ class DPMSolverSampler(SamplerBase):
     per step, so a run with the same seed consumes a different stream from theirs.
 
     eta > 0 (orders 1 and 2) is DPM-Solver++ 2M SDE (sde_coefficients, one glg_sde_update per step): it also draws one
-    randn_like(x) per step after the model pass, the last step included, after the blend's draw when there is a mask."""
+    randn_like(x) per step after the model pass, the last step included, after the blend's draw when there is a mask.
 
-    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2, eta=0.0):
+    grid="karras": the same draws, except that the last step (to sigma = 0) of an eta > 0 run draws no step noise: it is the
+    noiseless x_S = m_{S-1} (one glg_dpm_update).  The blend's draw is x0 alpha + sigma randn_like(x0), one per step with a mask,
+    as q_sample's.  The start state of image-to-image is alpha_0 init_latent + sigma_0 noise at the first point run."""
+
+    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2, eta=0.0,
+                 grid="ddim"):
         if order not in (1, 2, 3):
             raise ValueError(f"DPM-Solver++ order must be 1, 2 or 3, got {order!r}")
+        if grid not in GRIDS:
+            raise ValueError(f"grid must be one of {GRIDS}, got {grid!r}")
         if not 0.0 <= eta <= 1.0:
             raise ValueError(f"eta must lie in [0, 1], got {eta!r}")
         if eta > 0 and order == 3:
@@ -141,27 +182,30 @@ class DPMSolverSampler(SamplerBase):
         super().__init__(diffusion, model, schedule, alpha_generator_func, set_alpha_scale)
         self.order = order
         self.eta = float(eta)
+        self.grid = grid
+        self._grid = None                                       # the Karras SamplingGrid of the current sample() call
 
     @torch.no_grad()
     def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
         """init_latent / strength / noise: image-to-image, started part-way down the grid (SamplerBase._begin).  The (alpha,
-        sigma) grid is the truncated time steps plus alphas_cumprod[0]; step_orders lowers the orders at its start as usual."""
+        sigma) grid is the truncated time steps plus alphas_cumprod[0] (grid="ddim") or the last steps of the S-step Karras grid
+        (grid="karras"); step_orders lowers the orders at its start as usual."""
         self.make_schedule(ddim_num_steps=S)
+        self._grid = _karras.karras_grid(self.diffusion.alphas_cumprod, S) if self.grid == "karras" else None
         return self.dpm_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, init_latent=init_latent, strength=strength,
                                  noise=noise)
 
     @torch.no_grad()
     def dpm_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, init_latent=None, strength=1.0, noise=None):
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
-        if len(time_range) == 0:                                # strength 0: init_latent as it is
+        img, grid, alphas = self._begin(shape, input, init_latent, strength, noise, self._grid)
+        if len(grid.times) == 0:                                # strength 0: init_latent as it is
             return img
-        alpha, sigma = grid_alpha_sigma(self.diffusion.alphas_cumprod, time_range)
+        alpha, sigma = grid.alpha, grid.sigma
 
         def model_fn(i, x):
             self._apply_alpha(alphas, i)
-            ts = torch.full((b,), int(time_range[i]), device=self.device, dtype=torch.long)
-            x = self._inpaint_blend(x, mask, x0, ts)
+            x, ts = self._point(x, grid, i, b, mask, x0)
             input["x"], input["timesteps"] = x, ts
             e_c, e_u = self._eps_pair(input, uc, guidance_scale)
             return x, e_c, e_u
@@ -178,7 +222,10 @@ class DPMSolverSampler(SamplerBase):
                 input["x"] = x
                 return x
 
-            return sde_solve(img.contiguous().float(), alpha, sigma, self.order, self.eta, model_fn, sde_fn)
+            def final_fn(x, e_c, e_u, a, s, coefs, m0_out):
+                return update_fn(x, e_c, e_u, None, None, a, s, coefs, m0_out)
+
+            return sde_solve(img.contiguous().float(), alpha, sigma, self.order, self.eta, model_fn, sde_fn, final_fn)
         return dpm_solve(img.contiguous().float(), alpha, sigma, self.order, model_fn, update_fn)
 
     def _dpm_update(self, x, e_c, e_u, guidance_scale, m1, m2, alpha, sigma, coefs, m0_out):

@@ -23,7 +23,8 @@ class PLMSSampler(SamplerBase):
     @torch.no_grad()
     def plms_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, init_latent=None, strength=1.0, noise=None):
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
+        img, grid, alphas = self._begin(shape, input, init_latent, strength, noise)
+        time_range = grid.times
         total = len(time_range)                                 # step i runs at ddim_timesteps[total - i - 1]
         history = []                                            # newest first: e_{t-1}, e_{t-2}, e_{t-3}
         for i, step in enumerate(time_range):

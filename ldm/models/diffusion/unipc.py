@@ -7,7 +7,9 @@ data prediction with B(h) = expm1(-h) ("bh2"), with PLMSSampler's call surface p
 It steps on DPMSolverSampler's grid (the DDIM uniform grid, the last step to alphas_cumprod[0]) with its step orders, one UNet
 pass per step (one 2B pass when CFG is on): S = 10 costs 10 passes.  After each model evaluation the corrector UniC refines the
 state the model was evaluated at with the data prediction just computed, which costs no pass and raises the order by one; then
-the predictor UniP steps from the corrected state.  The last step is not corrected (that would need a pass at x_S).  UniP of
+the predictor UniP steps from the corrected state.  The last step is not corrected (that would need a pass at x_S).
+grid="karras" steps on the Karras sigma grid (_karras.py), as DPMSolverSampler's: S steps and S passes, fractional timesteps, and a
+final first-order step to sigma = 0, x_S = m_{S-1}; the predictor and corrector tables are unchanged on its lambda grid.  UniP of
 order 2 is DPM-Solver++ 2M.  Scheduled sampling, the first-conv swap and the inpainting blend are SamplerBase's; the blend
 replaces the point the model is evaluated at and reaches the corrected state only through that point's data prediction.  The
 CFG mix, the data prediction, the corrector and the predictor are one fp32 kernel per step (glg_unipc_update); the per-step
@@ -20,8 +22,9 @@ import torch
 
 from gligen_b200 import lib as _L
 
+from . import _karras
 from ._sampling import SamplerBase
-from .dpm_solver import grid_alpha_sigma, step_orders
+from .dpm_solver import GRIDS, grid_orders
 
 
 def _bh2_rhos(lam_t, lam_s, lam_hist, corrector):
@@ -82,6 +85,21 @@ def step_coefficients(alpha, sigma, orders):
     return out
 
 
+def grid_coefficients(alpha, sigma, orders):
+    """step_coefficients; when the grid ends at sigma = 0 (lambda = +inf) the final row's predictor is stated as x_S = m_{S-1},
+    (pc, p0, p1, p2) = (0, 1, 0, 0), and its corrector (of the state the final model pass saw) is the usual one."""
+    if sigma[-1] > 0.0:
+        return step_coefficients(alpha, sigma, orders)
+    n = len(orders)
+    a, s = np.asarray(alpha[:-1], dtype=np.float64), np.asarray(sigma[:-1], dtype=np.float64)
+    out = np.zeros((n, 9))
+    out[:-1] = step_coefficients(a, s, orders[:-1])
+    if n > 1:
+        out[-1, :5] = _expand(a, s, np.log(a) - np.log(s), n - 2, n - 1, orders[n - 2], corrector=True)
+    out[-1, 5:] = (0.0, 1.0, 0.0, 0.0)
+    return out
+
+
 def history_depth(orders, i):
     """How many earlier data predictions step i reads: m_{i-1} .. m_{i-depth}."""
     return max(orders[i - 1] if i > 0 else 0, orders[i] - 1)
@@ -93,8 +111,8 @@ def unipc_solve(x, alpha, sigma, order, model_fn, update_fn):
     m3, alpha_i, sigma_i, coefs, m_out, xc_out) -> x at point i + 1, writing this step's data prediction into m_out and its
     corrected state into xc_out (xc_prev None at i = 0: xc_0 = x_0).  The data predictions rotate through four buffers and the
     corrected states through two, allocated once: step i writes m buffer i % 4 and xc buffer i % 2 and reads the ones before."""
-    orders = step_orders(len(alpha) - 1, order)
-    coefs = step_coefficients(alpha, sigma, orders)
+    orders = grid_orders(sigma, order)
+    coefs = grid_coefficients(alpha, sigma, orders)
     hist = [torch.empty_like(x) for _ in range(4)]
     xcs = [torch.empty_like(x) for _ in range(2)]
     xc = None
@@ -111,34 +129,40 @@ def unipc_solve(x, alpha, sigma, order, model_fn, update_fn):
 class UniPCSampler(SamplerBase):
     """Generator draws: randn(shape) for x_T when input['x'] is None, and one randn_like per step for the q_sample noise of the
     inpainting blend when a mask is given.  With init_latent, randn(shape) for the noise of the start state in place of x_T, none
-    when the caller passes noise or no step runs.  Nothing else, as DPMSolverSampler."""
+    when the caller passes noise or no step runs.  Nothing else, as DPMSolverSampler.  grid="karras" draws the same; its blend
+    draw is x0 alpha + sigma randn_like(x0), as q_sample's."""
 
-    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2):
+    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None, order=2, grid="ddim"):
         if order not in (1, 2, 3):
             raise ValueError(f"UniPC order must be 1, 2 or 3, got {order!r}")
+        if grid not in GRIDS:
+            raise ValueError(f"grid must be one of {GRIDS}, got {grid!r}")
         super().__init__(diffusion, model, schedule, alpha_generator_func, set_alpha_scale)
         self.order = order
+        self.grid = grid
+        self._grid = None                                       # the Karras SamplingGrid of the current sample() call
 
     @torch.no_grad()
     def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, init_latent=None, strength=1.0, noise=None):
         """init_latent / strength / noise: image-to-image, started part-way down the grid (SamplerBase._begin).  The (alpha,
-        sigma) grid is the truncated time steps plus alphas_cumprod[0]; step_orders lowers the orders at its start as usual."""
+        sigma) grid is the truncated time steps plus alphas_cumprod[0] (grid="ddim") or the last steps of the S-step Karras grid
+        (grid="karras"); step_orders lowers the orders at its start as usual."""
         self.make_schedule(ddim_num_steps=S)
+        self._grid = _karras.karras_grid(self.diffusion.alphas_cumprod, S) if self.grid == "karras" else None
         return self.unipc_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, init_latent=init_latent, strength=strength,
                                    noise=noise)
 
     @torch.no_grad()
     def unipc_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, init_latent=None, strength=1.0, noise=None):
         b = shape[0]
-        img, time_range, alphas = self._begin(shape, input, init_latent, strength, noise)
-        if len(time_range) == 0:                                # strength 0: init_latent as it is
+        img, grid, alphas = self._begin(shape, input, init_latent, strength, noise, self._grid)
+        if len(grid.times) == 0:                                # strength 0: init_latent as it is
             return img
-        alpha, sigma = grid_alpha_sigma(self.diffusion.alphas_cumprod, time_range)
+        alpha, sigma = grid.alpha, grid.sigma
 
         def model_fn(i, x):
             self._apply_alpha(alphas, i)
-            ts = torch.full((b,), int(time_range[i]), device=self.device, dtype=torch.long)
-            x = self._inpaint_blend(x, mask, x0, ts)
+            x, ts = self._point(x, grid, i, b, mask, x0)
             input["x"], input["timesteps"] = x, ts
             e_c, e_u = self._eps_pair(input, uc, guidance_scale)
             return x, e_c, e_u

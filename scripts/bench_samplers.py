@@ -1,5 +1,6 @@
 """Images/s of the samplers on one GPU: PLMS-50 against DPM-Solver++ 2M at 20 and 25 steps, and UniPC-2 at 10 and 15 steps
-against DPM-Solver++ 2M at 10 (the same number of passes).
+against DPM-Solver++ 2M at 10 (the same number of passes); and on the Karras sigma grid (grid="karras"): 2M at 10 / 15 / 20 steps,
+UniPC-2 at 10 / 15 and 2M SDE (eta = 1) at 20.
 
     python scripts/bench_samplers.py [--repeats 2] [--batch 4]
 
@@ -11,10 +12,11 @@ alpha_type [0.3, 0, 0.7] (gligen_inference's default: the fusers are on for the 
    bound: x, e_c, e_u, m1 read and x0_out, x_prev written, over 3.35 TB/s (H100 SXM data sheet).  Likewise glg_unipc_update
    (order 3, a step that reads all three earlier data predictions): x, xc_prev, e_c, e_u, m1, m2, m3 read and m_out, xc_out,
    x_next written.  The UniPC rows must take exactly one UNet pass per image and step of the DDIM uniform grid (S of them, but
-   16 at S = 15: the grid's spacing is 1000 // S); the script stops if one does not.
+   16 at S = 15: the grid's spacing is 1000 // S); the Karras rows exactly S.  The script stops if one does not.
 3. A diagnostic, not a quality measure: the rel-L2 distance of each sampler's final latent from a DPM-Solver++ 3M run at 250
-   steps on the same seeded inputs.  That run is not a converged solution (the DDIM grid's last step, t = 1 -> alphas_cumprod[0],
-   has the same size at every S), and with synthetic weights the distance says how the solvers differ, not how the images look.
+   steps on the same seeded inputs, on the sampler's own grid.  The DDIM-grid run is not a converged solution (the grid's last
+   step, t = 1 -> alphas_cumprod[0], has the same size at every S); the Karras one shrinks every step.  With synthetic weights the
+   distance says how the solvers differ, not how the images look, and the SDE row's distance includes its own noise.
 Every run reloads the weights first (untimed), so each starts from the GLIGEN first conv like a fresh model.  The card's name and
 power limit are printed with the numbers.
 """
@@ -36,9 +38,15 @@ from bench_fusers import HBM_BYTES_PER_S, card  # noqa: E402
 
 DEV = "cuda:0"
 ALPHA_TYPE = [0.3, 0.0, 0.7]
-RUNS = [("PLMS-50", "plms", 50, None), ("DPM-Solver++ 2M-20", "dpm", 20, 2), ("DPM-Solver++ 2M-25", "dpm", 25, 2),
-        ("UniPC-2 10", "unipc", 10, 2), ("UniPC-2 15", "unipc", 15, 2), ("DPM-Solver++ 2M-10", "dpm", 10, 2)]
-REFERENCE_RUN = ("DPM-Solver++ 3M-250", "dpm", 250, 3)
+# (name, sampler, S, order, grid, eta); the Karras arms alternate with the DDIM-grid ones
+RUNS = [("PLMS-50", "plms", 50, None, "ddim", 0.0), ("DPM-Solver++ 2M Karras-10", "dpm", 10, 2, "karras", 0.0),
+        ("DPM-Solver++ 2M-20", "dpm", 20, 2, "ddim", 0.0), ("DPM-Solver++ 2M Karras-15", "dpm", 15, 2, "karras", 0.0),
+        ("DPM-Solver++ 2M-25", "dpm", 25, 2, "ddim", 0.0), ("DPM-Solver++ 2M Karras-20", "dpm", 20, 2, "karras", 0.0),
+        ("UniPC-2 10", "unipc", 10, 2, "ddim", 0.0), ("UniPC-2 Karras-10", "unipc", 10, 2, "karras", 0.0),
+        ("UniPC-2 15", "unipc", 15, 2, "ddim", 0.0), ("UniPC-2 Karras-15", "unipc", 15, 2, "karras", 0.0),
+        ("DPM-Solver++ 2M-10", "dpm", 10, 2, "ddim", 0.0), ("DPM-Solver++ 2M SDE Karras-20", "dpm", 20, 2, "karras", 1.0)]
+REFERENCE_RUNS = {"ddim": ("DPM-Solver++ 3M-250", "dpm", 250, 3, "ddim", 0.0),
+                  "karras": ("DPM-Solver++ 3M Karras-250", "dpm", 250, 3, "karras", 0.0)}
 
 
 def _graph_time(name, batch, launch, nbytes, reps=200):
@@ -133,15 +141,15 @@ def main():
     model.forward_cfg = counted
     kw = dict(alpha_generator_func=partial(alpha_generator, type=ALPHA_TYPE), set_alpha_scale=set_alpha_scale)
 
-    def run(kind, S, order):
+    def run(kind, S, order, grid, eta):
         model.load_state_dict(weights)
         model.engine()                                  # re-pack the weights outside the timed window
         if kind == "plms":
             sampler = PLMSSampler(diffusion, model, **kw)
         elif kind == "dpm":
-            sampler = DPMSolverSampler(diffusion, model, order=order, **kw)
+            sampler = DPMSolverSampler(diffusion, model, order=order, eta=eta, grid=grid, **kw)
         else:
-            sampler = UniPCSampler(diffusion, model, order=order, **kw)
+            sampler = UniPCSampler(diffusion, model, order=order, grid=grid, **kw)
         input, _, _ = sampler_inputs(cfg, model, dinp, dbatch)
         passes["n"] = 0
         torch.manual_seed(1234)
@@ -155,14 +163,14 @@ def main():
     os.chdir(os.path.join(ROOT, "tests", "golden"))     # restore_first_conv_from_SD reads SD_input_conv_weight_bias.pth CWD-relative
     try:
         latents, times, npass = {}, {name: [] for name, *_ in RUNS}, {}
-        for name, kind, S, order in RUNS:               # warm-up: every shape and schedule once
-            _, npass[name], latents[name] = run(kind, S, order)
-            steps = len(make_ddim_timesteps("uniform", S, 1000, verbose=False))
-            if kind == "unipc" and npass[name] != steps:
+        for name, kind, S, order, grid, eta in RUNS:    # warm-up: every shape and schedule once
+            _, npass[name], latents[name] = run(kind, S, order, grid, eta)
+            steps = S if grid == "karras" else len(make_ddim_timesteps("uniform", S, 1000, verbose=False))
+            if (kind == "unipc" or grid == "karras") and npass[name] != steps:
                 raise SystemExit(f"{name}: {npass[name]} UNet passes per image, expected one per step of the grid ({steps})")
         for _ in range(a.repeats):
-            for name, kind, S, order in RUNS:
-                secs, n, lat = run(kind, S, order)
+            for name, kind, S, order, grid, eta in RUNS:
+                secs, n, lat = run(kind, S, order, grid, eta)
                 times[name].append(secs)
                 if n != npass[name] or not torch.equal(lat, latents[name]):
                     print(f"{name}: a repeat run differs from the first ({n} passes)", flush=True)
@@ -176,12 +184,14 @@ def main():
         for name in results:
             results[name]["speedup_vs_plms50"] = results[name]["images_per_s"] / base
         if not a.no_reference_run:
-            name, kind, S, order = REFERENCE_RUN
-            _, n, ref = run(kind, S, order)
-            for k, lat in latents.items():
-                results[k]["rel_l2_vs_3m250"] = ((lat - ref).norm() / ref.norm()).item()
-                print(f"{k}: rel-L2 of the final latent from {name} = {results[k]['rel_l2_vs_3m250']:.3e} "
-                      "(solver diagnostic on synthetic weights, not an image-quality measure)", flush=True)
+            for grid, (name, *ref_run) in REFERENCE_RUNS.items():
+                _, n, ref = run(*ref_run)
+                for k, *_, g, _eta in RUNS:
+                    if g != grid:
+                        continue
+                    results[k]["rel_l2_vs_3m250"] = ((latents[k] - ref).norm() / ref.norm()).item()
+                    print(f"{k}: rel-L2 of the final latent from {name} = {results[k]['rel_l2_vs_3m250']:.3e} "
+                          "(solver diagnostic on synthetic weights, not an image-quality measure)", flush=True)
     finally:
         os.chdir(cwd)
     kern = update_kernel_time(a.batch)
